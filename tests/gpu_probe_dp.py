@@ -1,5 +1,5 @@
 """Development probe (not a pytest file): normal-mode parser kernel vs the oracle on a handful of inputs,
-with a symbol-trace diff on the first mismatch, and an A/B timing against the round-1 three-warp parser.
+with a symbol-trace diff on the first mismatch, and the parser's timing on a few multi-Block streams.
 
     python tests/gpu_probe_dp.py [quick|time|all]
 """
@@ -103,19 +103,13 @@ def timing():
     for kind, preset, nb, bs in (("T", 6, 8, 4 * MiB), ("E", 6, 8, 4 * MiB), ("E", 9 | EXT, 8, 2 * MiB)):
         n = nb * bs
         buf = X.gendata(kind, n)
-        for mode in ("dp", "warp3"):
-            if mode == "warp3":
-                os.environ["XZB_PARSE"] = "warp3"
-            else:
-                os.environ.pop("XZB_PARSE", None)
-            ctx = xz_b200.Context(0)
-            o = xz_b200.lzma_lzma_preset(preset)
-            ctx.stream_encode(buf, preset=preset, block_size=bs, n=n, opts=o)
-            ctx.stream_encode(buf, preset=preset, block_size=bs, n=n, opts=o)
-            s = ctx.stats().as_dict()
-            print(f"time {kind} -{preset & 31} {nb}x{bs // MiB}MiB {mode}: parse_ms={s['ms_parse']:.1f} mf_ms={s['ms_mf']:.1f} total_ms={s['ms_total']:.1f}", flush=True)
-            ctx.close()
-        os.environ.pop("XZB_PARSE", None)
+        ctx = xz_b200.Context(0)
+        o = xz_b200.lzma_lzma_preset(preset)
+        ctx.stream_encode(buf, preset=preset, block_size=bs, n=n, opts=o)
+        ctx.stream_encode(buf, preset=preset, block_size=bs, n=n, opts=o)
+        s = ctx.stats().as_dict()
+        print(f"time {kind} -{preset & 31} {nb}x{bs // MiB}MiB: parse_ms={s['ms_parse']:.1f} mf_ms={s['ms_mf']:.1f} total_ms={s['ms_total']:.1f}", flush=True)
+        ctx.close()
 
 
 if __name__ == "__main__":

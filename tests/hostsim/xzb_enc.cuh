@@ -1,6 +1,7 @@
 // xzb_enc.cuh -- LZMA symbol selection + range coding + LZMA2 chunking for one .xz block, single-thread form.
 // TEST HARNESS ONLY (tests/hostsim): the sequential statement of the encoder that the host simulation checks against
-// the oracle; the product library contains the warp designs (xzb_parse_dp.cuh, xzb_parse_warp.cuh) only.
+// the oracle; the product library contains the warp designs only (normal mode: xzb_parse_dp.cuh, fast mode and
+// the coder both share: xzb_parse_warp.cuh).
 //
 // This is the strictly sequential half of the encoder (probabilities, price tables, reps and
 // state all depend on every earlier symbol).  One CUDA block owns one .xz block; matches

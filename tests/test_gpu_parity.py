@@ -191,10 +191,9 @@ def test_normal_mode_multi_block_properties(ctx, kind):
     assert r == 0 and back == bytes(buf[:n])
 
 
-def test_multiple_waves_and_both_normal_mode_kernels_agree(monkeypatch):
+def test_multiple_waves_give_the_same_bytes(monkeypatch):
     """Streams longer than one wave are encoded wave by wave (XZB_MAX_WAVE_BLOCKS forces 2-block waves
-    here); bytes must not depend on the wave size.  Also cross-checks the round-1 three-warp parser
-    (XZB_PARSE=warp3, an independent implementation of lzma_lzma_optimum_normal) against the oracle."""
+    here); bytes must not depend on the wave size."""
     import xz_b200
     n, bs = 5 * 262144 + 1234, 262144
     buf = X.gendata("E", n)
@@ -206,13 +205,25 @@ def test_multiple_waves_and_both_normal_mode_kernels_agree(monkeypatch):
         assert c.stats().n_blocks == 6
     finally:
         c.close()
-    monkeypatch.delenv("XZB_MAX_WAVE_BLOCKS")
-    monkeypatch.setenv("XZB_PARSE", "warp3")
-    c = xz_b200.Context(0)
-    try:
-        assert c.stream_encode(buf, preset=6, block_size=bs, n=300000) == X.oracle_encode(buf, 300000, 6, bs)
-    finally:
-        c.close()
+
+
+def test_fast_mode_kernel_forms_match_oracle(ctx):
+    """Fast mode (presets 0-3) runs in one of two launch forms, chosen per wave: a wave with more Blocks than
+    the GPU has SMs (400 here, more than any H100 has) packs several Blocks per SM with a coder warp for the
+    range coder; a wave of a few Blocks gives every Block an SM to itself.  Both must give the oracle's bytes,
+    for hash chains (presets 1 and 3) and for a binary tree (BT4)."""
+    import xz_b200
+    bt4 = xz_b200.lzma_lzma_preset(2)
+    bt4.mf, bt4.nice_len, bt4.depth = 0x14, 64, 0
+    xbt4 = X.preset_options(2); xbt4.mf, xbt4.nice_len, xbt4.depth = 0x14, 64, 0
+    for nblocks, bs in ((400, 4096), (3, 1 << 17)):
+        n = nblocks * bs - 123   # short last Block
+        for kind, preset in (("T", 1), ("R", 1), ("T", 3), ("R", 3)):
+            buf = X.gendata(kind, n)
+            assert ctx.stream_encode(buf, preset=preset, block_size=bs, n=n) == X.oracle_encode(buf, n, preset, bs), (nblocks, kind, preset)
+        buf = X.gendata("T", n)
+        assert ctx.stream_encode(buf, opts=bt4, block_size=bs, n=n) == X.oracle_encode(buf, n, 2, bs, opts=xbt4), (nblocks, "bt4")
+        assert ctx.stats().n_blocks == nblocks
 
 
 @pytest.mark.parametrize("seg_shift,overlap", [(8, 1), (10, 1), (12, 0), (16, 1), (20, 0)])

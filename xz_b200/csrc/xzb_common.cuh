@@ -69,7 +69,7 @@
 #define XZB_DATA_ERROR 9
 #define XZB_BUF_ERROR 10
 #define XZB_PROG_ERROR 11
-#define XZB_MF_STALL 102            // internal: parser watchdog, see WarpEnc::mf_wait
+#define XZB_MF_STALL 102            // internal: parser watchdog, see WarpEncT::mf_wait
 #define XZB_MF_STALL_NS 30000000000ull  // no match-finder progress for this long = kernels are not running side by side
 
 typedef uint16_t xzb_prob;

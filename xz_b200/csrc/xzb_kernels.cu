@@ -6,7 +6,7 @@
 //   radix sort + xzb_k_prev                 : previous occurrence per hash = the hash heads
 //   xzb_k_hc | xzb_k_bt                     : match finder -> match store (HBM)
 //   xzb_k_crc                               : CRC64/CRC32 of every block (slice + GF(2) fold)
-//   xzb_k_parse_dp | xzb_k_parse_fast | xzb_k_parse_warp  1 CUDA block / .xz block : parser + range coder + LZMA2 chunker
+//   xzb_k_parse_dp | xzb_k_parse_fast  1 CUDA block / .xz block : parser + range coder + LZMA2 chunker
 //   xzb_k_finalize    1 CUDA block / .xz block : header, padding, check | raw fallback
 // Decode: xzb_k_decode (1 CUDA block / .xz block) + xzb_k_crc over the output.
 // There is deliberately no CPU path in this file.
@@ -260,97 +260,64 @@ struct XzbEncJob {
 	uint64_t fit_limit;      // see xzb_block_finish_normal
 };
 
-// Production parser: one CUDA block per .xz block, all coder state in shared memory
-// (xzb_parse_warp.cuh).  Warp 0 = DP front half + range coder, warp 1 = helper that prepares the
-// state-independent match candidates of the positions ahead, warp 2 = back half of helper2 one
-// position behind warp 0 (warps 1 and 2: normal mode only).
+// Parser kernels: one CUDA block per .xz block, all coder state in shared memory (xzb_parse_warp.cuh,
+// xzb_parse_dp.cuh).  The coding warp and the warps that work for it share these parameters.
 template <class ENC>
 static __device__ void xzb_setup_warp(ENC &E, const XzbEncJob &job, const XzbMfBlock &blk, const XzbParams &P)
 {
 	E.buf = blk.buf; E.size = job.in_size;   // the bytes LZMA2 codes (after Delta / BCJ); job.in stays the unfiltered input
 	E.g_mh = blk.mh; E.g_mp = blk.mp; E.g_ovf = blk.ovf;
 	E.read_pos = 0; E.read_ahead = 0; E.ring_base = 0x80000000u;
-	E.nice_len = P.nice_len; E.fast_mode = P.mode == XZB_MODE_FAST;
+	E.nice_len = P.nice_len;
 	E.pos_mask = (1u << P.pb) - 1; E.lc = P.lc; E.literal_mask = (0x100u << P.lp) - (0x100u >> P.lc);
 	E.dist_table_size = P.dist_table_size; E.len_table_size = P.len_table_size; E.num_pos_states = 1u << P.pb;
 	E.uncomp_size = 0; E.is_initialized = 0; E.n_symbols = 0; E.matches_count = 0; E.longest_match_length = 0;
-	E.h_r0 = E.h_r1 = E.h_r2 = E.h_r3 = 0;
 	E.rc_out = job.out; E.rc_out_pos = 0;
-	E.use_mwarp = !E.fast_mode;
-	E.bw_posted = 0;
 }
 
+// Dynamic shared memory of the two-warp fast-mode form.  Its state needs only sizeof(FS<false>), but each Block of a wave
+// that leaves SMs idle gets an SM to itself: more than half of an SM's 228 KB leaves no room for a second parser CTA, so
+// the B parser CTAs take B SMs and the match finder beside them counts on the other sm_count - B (`avoid`, encode_wave).
+// Above 196 KB the SM also keeps the shared-memory / L1 split that the normal-mode kernel (sizeof(DS)) runs with.
+#define XZB_SOLO_SMEM (220u * 1024u)
+
+// Fast mode (presets 0-3): three warps per .xz Block.
+//   warp 1  decisions: lzma_lzma_optimum_fast looks only at the match store, the window and the reps, so it runs ahead;
+//   warp 0  coding: resolves every symbol's probability indices in closed form, adapts the probabilities, LZMA2 chunker;
+//   warp 2  CODER_WARP: range coder arithmetic + byte output (xzb_w_coder_main), fed through a ring of (probability, bit)
+//           records; otherwise warp 0 runs the range coder itself and warp 2 returns at once.
+// The host picks the form per wave (see launch_parse).  The coder-warp form is launched with sizeof(FS<true>), so several
+// Blocks share an SM; the two-warp form with XZB_SOLO_SMEM.
+template <bool CODER_WARP>
 __global__ void __launch_bounds__(96)
-xzb_k_parse_warp(const XzbEncJob *__restrict__ jobs, const XzbMfBlock *__restrict__ blocks, XzbParams P,
-		const uint8_t *__restrict__ price_table, const uint32_t *mf_flag, uint32_t *parser_sm, uint64_t mf_stall_ns,
-		XzbBlockResult *__restrict__ results, uint32_t *__restrict__ payload_end)
+xzb_k_parse_fast(const XzbEncJob *__restrict__ jobs, const XzbMfBlock *__restrict__ blocks, XzbParams P,
+		const uint32_t *mf_flag, uint32_t *parser_sm, uint64_t mf_stall_ns, XzbBlockResult *__restrict__ results, uint32_t *__restrict__ payload_end)
 {
 	extern __shared__ __align__(16) uint8_t xzb_smem[];
-	WS &S = *reinterpret_cast<WS *>(xzb_smem);
+	FS<CODER_WARP> &S = *reinterpret_cast<FS<CODER_WARP> *>(xzb_smem);
 	const uint32_t lane = threadIdx.x & 31;
 	const uint32_t warp = threadIdx.x >> 5;
 	const uint32_t b = blockIdx.x;
 	const XzbEncJob job = jobs[b];
-	for (uint32_t i = threadIdx.x; i < 128; i += 96) S.prices[i] = price_table[i];
 	if (threadIdx.x == 0) {
 		uint32_t smid;
 		asm volatile("mov.u32 %0, %%smid;" : "=r"(smid));
 		if (smid < 256) ((volatile uint32_t *)parser_sm)[smid] = 1;  // the match finder's CTAs keep off this SM (xzb_k_bt)
 	}
 	if (threadIdx.x < XZB_FRING) S.f_tag[threadIdx.x] = 0;
-	if (threadIdx.x == 0) { S.f_epoch = 0; S.f_start_pos = 0; S.f_consumed = 0; S.m_epoch = 0; S.m_consumed = 0; S.m_exit = 0; S.m_pos0 = 0; S.m_position0 = 0; S.bw_go = 0; S.bw_done = 0; S.bw_len_end = 0; }
-	if (threadIdx.x < MREC_RING) S.mrec[threadIdx.x].tag = 0;
-	__syncthreads();
-	WarpEnc E(S, lane);
-	xzb_setup_warp(E, job, blocks[b], P);
-	E.mf_flag = mf_flag; E.mf_done = 0; E.mf_stall_ns = mf_stall_ns;
-	if (warp == 1) {
-		if (E.use_mwarp) xzb_w_helper_main(S, E);
-		else xzb_w_fast_parser_main(S, E);
-		return;
-	}
-	if (warp == 2) {
-		if (E.use_mwarp) xzb_w_back_main(S, E);
-		return;
-	}
-	E.reset();
-	uint32_t out_pos = job.header_size, ncl = 0, ncr = 0;
-	const int ret = xzb_w_lzma2_encode_block(E, P, job.out, job.out_cap, &out_pos, &ncl, &ncr);
-	if (lane == 0) {
-		S.m_exit = 1;
-		XzbBlockResult *res = results + b;
-		res->ret = (uint32_t)ret;
-		res->n_symbols = E.n_symbols; res->n_chunks_lzma = ncl; res->n_chunks_raw = ncr;
-		payload_end[b] = out_pos;
-	}
-}
-
-// Fast mode (presets 0-3): three warps per .xz Block, 36 KB of shared memory, several Blocks per SM.
-//   warp 1  decisions: lzma_lzma_optimum_fast looks only at the match store, the window and the reps, so it runs ahead;
-//   warp 0  coding: resolves every symbol's probability indices in closed form, adapts the probabilities, LZMA2 chunker;
-//   warp 2  range coder arithmetic + byte output (xzb_w_coder_main), fed through a ring of (probability, bit) records.
-// XZB_FAST=warp2 selects the round-1 two-warp form inside xzb_k_parse_warp (A/B).
-__global__ void __launch_bounds__(96)
-xzb_k_parse_fast(const XzbEncJob *__restrict__ jobs, const XzbMfBlock *__restrict__ blocks, XzbParams P,
-		const uint32_t *mf_flag, uint64_t mf_stall_ns, XzbBlockResult *__restrict__ results, uint32_t *__restrict__ payload_end)
-{
-	extern __shared__ __align__(16) uint8_t xzb_smem[];
-	FS &S = *reinterpret_cast<FS *>(xzb_smem);
-	const uint32_t lane = threadIdx.x & 31;
-	const uint32_t warp = threadIdx.x >> 5;
-	const uint32_t b = blockIdx.x;
-	const XzbEncJob job = jobs[b];
-	if (threadIdx.x < XZB_FRING) S.f_tag[threadIdx.x] = 0;
 	if (threadIdx.x == 0) {
 		S.f_epoch = 0; S.f_start_pos = 0; S.f_consumed = 0; S.m_exit = 0;
 		S.rcq_head = 0; S.rcq_tail = 0; S.rcq_T = 1; S.rcq_flushes = 0; S.rcq_out_pos = 0; S.rcq_out = nullptr;
 	}
 	__syncthreads();
-	WarpEncT<FS> E(S, lane);
+	WarpEncT<FS<CODER_WARP>> E(S, lane);
 	xzb_setup_warp(E, job, blocks[b], P);
 	E.mf_flag = mf_flag; E.mf_done = 0; E.mf_stall_ns = mf_stall_ns;
 	if (warp == 1) { xzb_w_fast_parser_main(S, E); return; }
-	if (warp == 2) { xzb_w_coder_main(S, E); return; }
+	if (warp == 2) {
+		if constexpr (CODER_WARP) xzb_w_coder_main(S, E);
+		return;
+	}
 	E.reset();
 	uint32_t out_pos = job.header_size, ncl = 0, ncr = 0;
 	const int ret = xzb_w_lzma2_encode_block(E, P, job.out, job.out_cap, &out_pos, &ncl, &ncr);
@@ -577,11 +544,8 @@ struct xzb_ctx {
 	bool overlap = true;                // XZB_OVERLAP=0, or a profiler/sanitizer that serialises kernels, turns it off
 	uint32_t seg_shift = 20;            // XZB_SEG_SHIFT
 	bool avoid_parser_sms = true;       // XZB_MF_AVOID_PARSER_SMS
-	bool parse_first = false;           // XZB_PARSE_FIRST=1: search kernels enqueued after the parser kernel did not start beside it (DESIGN.md)
 	uint64_t mf_stall_ns = XZB_MF_STALL_NS;  // XZB_MF_STALL_MS
 	uint32_t mf_stalls = 0;
-	bool parse_warp3 = false;  // XZB_PARSE=warp3: round-1 three-warp parser for normal mode (A/B)
-	int fast_form = 0;         // XZB_FAST=warp2 | small: force the fast-mode kernel (default: by Blocks per wave, see launch_parse)
 	const char *trace_path = nullptr;  // XZB_TRACE=file: symbol trace of block 0 of every wave (normal mode, debugging aid)
 	DevBuf trace;
 	uint32_t max_wave_blocks = 0;
@@ -664,8 +628,6 @@ extern "C" int xzb_ctx_create(xzb_ctx **out, int device)
 			ctx->overlap = false;
 		const char *av = getenv("XZB_MF_AVOID_PARSER_SMS");
 		if (av) ctx->avoid_parser_sms = atoi(av) != 0;
-		const char *pf = getenv("XZB_PARSE_FIRST");
-		if (pf) ctx->parse_first = atoi(pf) != 0;
 		const char *sm = getenv("XZB_MF_STALL_MS");
 		if (sm) ctx->mf_stall_ns = (uint64_t)std::max(100, atoi(sm)) * 1000000ull;
 		const char *ss = getenv("XZB_SEG_SHIFT");
@@ -673,17 +635,14 @@ extern "C" int xzb_ctx_create(xzb_ctx **out, int device)
 	}
 	xzb_make_tables(&ctx->h_tab);
 	{
-		const char *pv = getenv("XZB_PARSE");
-		ctx->parse_warp3 = pv && strcmp(pv, "warp3") == 0;
-		{ const char *fv = getenv("XZB_FAST"); ctx->fast_form = fv && strcmp(fv, "warp2") == 0 ? 1 : fv && strcmp(fv, "small") == 0 ? 2 : 0; }
-		cudaFuncSetAttribute(xzb_k_parse_fast, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(FS));
+		cudaFuncSetAttribute(xzb_k_parse_fast<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(FS<true>));
 		ctx->trace_path = getenv("XZB_TRACE");
 		const char *mw = getenv("XZB_MAX_WAVE_BLOCKS");
 		ctx->max_wave_blocks = mw ? (uint32_t)atoi(mw) : 0;
 		cudaFuncSetAttribute(xzb_k_decode, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(XzbDec));
 		if (cudaFuncSetAttribute(xzb_k_parse_dp, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(DS)) != cudaSuccess
-				|| cudaFuncSetAttribute(xzb_k_parse_warp, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(WS)) != cudaSuccess) {
-			fprintf(stderr, "xzb200: cannot reserve %zu B of shared memory for the parser kernel\n", sizeof(WS));
+				|| cudaFuncSetAttribute(xzb_k_parse_fast<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)XZB_SOLO_SMEM) != cudaSuccess) {
+			fprintf(stderr, "xzb200: cannot reserve %zu B of shared memory for the parser kernel\n", sizeof(DS));
 			delete ctx; return XZB_PROG_ERROR;
 		}
 	}
@@ -987,20 +946,19 @@ static int encode_wave(xzb_ctx *ctx, const uint8_t *d_in, uint64_t in_bytes, boo
 		d_trace = (uint32_t *)ctx->trace.p + 1;
 	}
 	auto launch_parse = [&]() {
-		if (P.mode == XZB_MODE_NORMAL && !ctx->parse_warp3) {
+		if (P.mode == XZB_MODE_NORMAL) {
 			xzb_k_parse_dp<<<B, P.nice_len > 127 ? 224 : 512, sizeof(DS), st>>>(d_jobs, d_blocks, P, ctx->d_prices, d_flag, d_parser_sm, ctx->mf_stall_ns, d_results, d_pend,
 					d_trace, trace_cap);
-		} else if (P.mode == XZB_MODE_FAST && (ctx->fast_form == 2 || (ctx->fast_form == 0 && B > (uint32_t)ctx->sm_count))) {
-			// Fast mode has two forms.  With more Blocks in the wave than SMs the 36 KB kernel runs (six Blocks per SM,
-			// measured 24 % slower per Block on 8 x 4 MiB `T` at -1 but up to six times the Blocks in flight); a wave that
-			// leaves SMs idle anyway keeps the two-warp form inside xzb_k_parse_warp.
-			xzb_k_parse_fast<<<B, 96, sizeof(FS), st>>>(d_jobs, d_blocks, P, d_flag, ctx->mf_stall_ns, d_results, d_pend);
+		} else if (B > (uint32_t)ctx->sm_count) {
+			// Fast mode has two forms.  With more Blocks in the wave than SMs the coder-warp form runs at its own size, so
+			// several Blocks share an SM (measured 24 % slower per Block on 8 x 4 MiB `T` at -1, but several times the
+			// Blocks in flight); a wave that leaves SMs idle anyway runs the two-warp form, one Block per SM.
+			xzb_k_parse_fast<true><<<B, 96, sizeof(FS<true>), st>>>(d_jobs, d_blocks, P, d_flag, d_parser_sm, ctx->mf_stall_ns, d_results, d_pend);
 		} else {
-			xzb_k_parse_warp<<<B, 96, sizeof(WS), st>>>(d_jobs, d_blocks, P, ctx->d_prices, d_flag, d_parser_sm, ctx->mf_stall_ns, d_results, d_pend);
+			xzb_k_parse_fast<false><<<B, 96, XZB_SOLO_SMEM, st>>>(d_jobs, d_blocks, P, d_flag, d_parser_sm, ctx->mf_stall_ns, d_results, d_pend);
 		}
 		++launches;
 	};
-	bool parse_launched = false;
 	if (!P.is_bt) {
 		dim3 grid((bs + 127) / 128, B);
 		xzb_k_hc<<<grid, 128, 0, st>>>(d_blocks, P);
@@ -1012,14 +970,6 @@ static int encode_wave(xzb_ctx *ctx, const uint8_t *d_in, uint64_t in_bytes, boo
 		// oversubscribed by the CTAs that will retire there, `live` CTAs do the work.
 		const bool avoid = overlap && ctx->avoid_parser_sms && (uint32_t)ctx->sm_count >= B + 16;
 		const uint32_t mf_sms = avoid ? (uint32_t)ctx->sm_count - B : (uint32_t)ctx->sm_count;
-		if (overlap && ctx->parse_first) {
-			// the parser CTAs take their SMs first and poll the progress flag; the search kernels fill the rest
-			launch_crc();
-			CK(cudaEventRecord(ctx->ev[3], st));
-			launch_parse();
-			CK(cudaEventRecord(ctx->ev[4], st));
-			parse_launched = true;
-		}
 		if (overlap) CK(cudaStreamWaitEvent(st_mf, ctx->ev[1], 0));
 		CK(cudaEventRecord(ctx->ev_mf[0], st_mf));
 		int per_sm = 0;
@@ -1041,17 +991,12 @@ static int encode_wave(xzb_ctx *ctx, const uint8_t *d_in, uint64_t in_bytes, boo
 		// SHA-256 needs only the input: behind the search on its stream, i.e. beside the parser when overlapping
 		if (check == 10) { xzb_k_sha256<<<B, 32, 0, st_mf>>>(d_crcjobs, (uint8_t *)d_crcv); ++launches; CK(cudaEventRecord(ctx->ev_mf[2], st_mf)); }
 	}
-	if (!parse_launched) {
-		launch_crc();
-		CK(cudaEventRecord(ctx->ev[3], st));
-	}
+	launch_crc();
+	CK(cudaEventRecord(ctx->ev[3], st));
 	results.resize(B);
 	for (int attempt = 0;; ++attempt) {
-		if (!parse_launched) {
-			launch_parse();
-			CK(cudaEventRecord(ctx->ev[4], st));
-		}
-		parse_launched = false;
+		launch_parse();
+		CK(cudaEventRecord(ctx->ev[4], st));
 		if (P.is_bt && overlap) CK(cudaStreamWaitEvent(st, check == 10 ? ctx->ev_mf[2] : ctx->ev_mf[1], 0));  // also: workspace is reused by the next wave
 		xzb_k_finalize<<<B, 256, 0, st>>>(d_jobs, ctx->d_crc32, P, check, (const uint8_t *)d_crcv, d_pend, d_results);
 		++launches;
@@ -1678,5 +1623,6 @@ extern "C" int xzb_stream_decode_prior(xzb_ctx *ctx, const uint8_t *in, uint64_t
 	return ret;
 }
 
-static_assert(sizeof(WS) <= 227 * 1024, "parser shared memory exceeds the 227 KB per-CTA limit of sm_90");
+static_assert(sizeof(FS<false>) <= XZB_SOLO_SMEM && 2 * XZB_SOLO_SMEM > 228 * 1024 && XZB_SOLO_SMEM <= 227 * 1024,
+		"the two-warp fast-mode kernel must hold its state and take more than half of an SM's 228 KB of shared memory");
 static_assert(sizeof(DS) <= 227 * 1024, "parser shared memory exceeds the 227 KB per-CTA limit of sm_90");

@@ -35,12 +35,8 @@
 // Reader: flag (volatile), DP_ACQUIRE(), data -- the loads are control-dependent on the flag, the barrier only
 // keeps the compiler from hoisting them.  The writer needs no fence.cta either: a warp's shared-memory stores are
 // performed in program order by the SM's in-order shared-memory pipeline, and a fence would wait for every store in
-// flight; XZB_DP_FENCED (A/B switch) puts the fence back.
-#ifdef XZB_DP_FENCED
-#define DP_RELEASE() __threadfence_block()
-#else
+// flight (DESIGN.md section 8 lists the fence among the dead ends).
 #define DP_RELEASE() asm volatile("" ::: "memory")
-#endif
 #define DP_ACQUIRE() asm volatile("" ::: "memory")
 #ifdef XZB_DP_PROF
 #define DP_T(v) const long long v = clock64()
@@ -67,9 +63,7 @@ __device__ __forceinline__ void dp_sts128(volatile void *p, const uint4 v)
 
 // The owner of node c looks at slot c once node c - DP_PEEK_LAG is final.  With lag 1 the record is late for a large
 // share of the nodes; with lag 2 it is not, and the candidate that leads the slot then is nearly always the final winner.
-#ifndef DP_PEEK_LAG
 #define DP_PEEK_LAG 2u
-#endif
 #define DP_WMAX 12u
 #define DP_POOL 3088u                 // ring slots: 12 workers x (256 + 1) or 3 workers x (1024 + 1); +1 skews the rings over the banks
 #define DP_NR 1024u                   // node-record / phase-flag ring capacity (>= ring size)
@@ -96,7 +90,7 @@ typedef uint4 DpPrep;
 #define DP_RCQ 2048u                  // coded-bit ring to the coder warp (16-bit records)
 struct DS {  // dynamic shared memory of xzb_k_parse_dp
 	static constexpr uint32_t RCQ = DP_RCQ;
-	static constexpr bool FAST_ONLY = false;
+	static constexpr bool FAST = false;
 	// ---- coder state shared with WarpEncT's methods ----
 	uint32_t len_prices[2][XZB_POS_STATES_MAX][XZB_LEN_SYMBOLS];
 	uint32_t dist_slot_prices[XZB_DIST_STATES][XZB_DIST_SLOTS];
@@ -150,7 +144,6 @@ struct DpEnc : WarpEncT<DS> {
 	__device__ DpEnc(DS &s, uint32_t l) : WarpEncT<DS>(s, l) {}
 
 	__device__ void reset() { WarpEncT<DS>::reset(); sym_cur = sym_end = 0; }  // lzma_lzma_encoder_reset: opts_*_index = 0
-	__device__ __forceinline__ void fast_restart(uint32_t) {}   // fast mode never runs on this kernel
 	__device__ __forceinline__ uint2 *sym_stack() const { return reinterpret_cast<uint2 *>(&S.ring_pool[0]); }  // 4096 x {back, len}
 	static __device__ __forceinline__ uint32_t st_lit(uint32_t s) { return s <= 3 ? 0 : (s <= 9 ? s - 3 : s - 6); }
 	static __device__ __forceinline__ uint32_t tagn(uint32_t ep, uint32_t node) { return ((ep & 0x3FFFu) << 16) | node; }
@@ -742,11 +735,7 @@ __device__ inline void xzb_dp_worker_main(DS &S, DpEnc &H, const uint32_t w)
 			// bundle.  The chain warp uses the record only if that very candidate wins the slot in the end.
 			bool have_p = false;              // window compare done ahead for the predicted reps rp_*
 			uint32_t rmaskb_p = 0, cvw_p = 0, rp_0 = 0, rp_1 = 0, rp_2 = 0, rp_3 = 0;
-#ifdef XZB_DP_NO_PEEK
-			if (false) {
-#else
 			if (c >= 3) {
-#endif
 				// (every decision in these polling loops is lane 0's, broadcast: lanes that reach a loop at different times must
 				// not leave it on different values of a flag that changes meanwhile -- the collectives below need the whole warp)
 				uint32_t fnode = 0;
@@ -847,11 +836,7 @@ __device__ inline void xzb_dp_worker_main(DS &S, DpEnc &H, const uint32_t w)
 				const bool lr_near = (mg0 & 0xF) == 0x9;
 				{
 					const bool other_reps = ((rmaskb >> 8) & 3) == 0 || ((rmaskb >> 16) & 3) == 0 || ((rmaskb >> 24) & 3) == 0;
-#ifdef XZB_DP_NO_NEAR
-					if (false) {
-#else
 					if (!other_reps && nice_len >= 8 && count <= 32) {
-#endif
 						const uint32_t L2 = lane + 2;
 						const bool eqL = lane == 0 ? (mg0 & 3) == 0 : (mg0 & 7) == 0;
 						const bool vr = lane < 2 && eqL, vmn = lane < 2 && !eqL && L2 <= new_len;

@@ -1,18 +1,18 @@
-// xzb_parse_warp.cuh -- warp-cooperative LZMA parser + range coder (device only).
+// xzb_parse_warp.cuh -- warp-cooperative LZMA coder + the fast-mode parser (device only).
 //
 // Same decisions, bit for bit, as the sequential restatement in xzb_enc.cuh (which stays in the
 // tree as the single-thread form that tests/hostsim checks against the oracle), but organised
-// for one warp per .xz block with every piece of coder state in shared memory:
-//   * probability model, price tables and the whole opts[4096] DP array live in smem (SoA);
+// for one CUDA block per .xz block with every piece of coder state in shared memory.  WarpEncT is
+// the part both parsers share: probability model, price tables, match store reader, symbol
+// encoder, range coder and the LZMA2 chunker.  The normal-mode parser (presets 4-9) builds on it
+// in xzb_parse_dp.cuh; fast mode (presets 0-3) is complete here:
 //   * match lists stream from the HBM match store through a 32-position smem ring filled with
 //     coalesced 16 B loads;
-//   * inside one DP position the lanes are the candidate lengths / tree levels / compared bytes
-//     (ballot + ffs memcmplen, redux literal prices, one lane per len_test);
+//   * lzma_lzma_optimum_fast needs no coder state, so its decisions are taken by a warp of their
+//     own ahead of the coding warp (xzb_w_fast_parser_main);
 //   * an LZMA symbol's probability indices are computed in closed form by the lanes, the
 //     adaptive-probability updates happen in parallel, and only the low/range recurrence of the
-//     range coder runs serially in lane 0.
-// Candidate application order follows the reference's program order wherever two candidates can
-// hit the same opts[] slot with equal price (strict '<' keeps the first), see w_helper2.
+//     range coder runs serially (on the coding warp, or on a coder warp: see FS).
 #pragma once
 #include "xzb_common.cuh"
 #include "xzb_mf.cuh"
@@ -40,82 +40,13 @@
 #define LC_MID 130
 #define LC_HIGH 258
 
-// Everything of DP position `cur` that the later parts of helper2 need (see WarpEnc::h2_front).
-struct H2 {
-	uint32_t cur, position, bpos, buf_avail_full, buf_avail;
-	uint32_t st, hr[4], cur_price, rmask, current_byte, match_byte, pos_state;
-	uint32_t cur_and_1_price, match_price, rep_match_price, next_is_literal;
-	uint32_t mcount, new_len;
-};
-
-#define MREC_RING 8
-// One position's match candidates with everything that does not depend on the DP state folded in:
-// plain_rel[l-2] = get_dist_len_price(dist of the match covering l, l, pos_state); m_rel[i] = price of
-// "match i + literal + rep0" minus (normal_match_price + is_match[state_after_match] bit).
-struct MRec {
-	volatile uint32_t tag;  // (epoch << 16 | k) + 1 once the record is complete
-	uint16_t count, longest, nplain, slow;
-	uint16_t m_len[8], m_lt2[8];
-	uint32_t m_dist[8], m_rel[8];
-	uint32_t plain_rel[XZB_MATCH_LEN_MAX - 1];
-	uint8_t plain_i[XZB_MATCH_LEN_MAX + 1];
-};
-
 #define XZB_MF_MARGIN 96u
 #define XZB_FRING 64u
 #define XZB_BACK_STALL 0xFFFFFFFEu  // ring entry: the parser warp's match-finder watchdog fired
 
-struct WS {  // dynamic shared memory of xzb_k_parse_warp
-	static constexpr uint32_t RCQ = 0;   // the range coder runs on the coding warp itself (see DS::RCQ)
-	static constexpr bool FAST_ONLY = false;
-	uint32_t o_price[XZB_OPTS], o_back_prev[XZB_OPTS], o_back_prev_2[XZB_OPTS];
-	uint4 o_backs[XZB_OPTS];
-	uint16_t o_pos_prev[XZB_OPTS], o_pos_prev_2[XZB_OPTS];
-	uint8_t o_state[XZB_OPTS], o_flags[XZB_OPTS];  // flags: bit0 prev_1_is_literal, bit1 prev_2
-	uint32_t len_prices[2][XZB_POS_STATES_MAX][XZB_LEN_SYMBOLS];  // [0] match, [1] rep
-	uint32_t dist_slot_prices[XZB_DIST_STATES][XZB_DIST_SLOTS];
-	uint32_t dist_prices[XZB_DIST_STATES][XZB_FULL_DISTANCES];
-	uint32_t align_prices[XZB_ALIGN_SIZE];
-	uint32_t len_counters[2][XZB_POS_STATES_MAX];
-	alignas(16) xzb_pair ring_mp[32][8];
-	uint32_t ring_mh[32];
-	uint32_t m_dist[XZB_MATCH_LEN_MAX + 1];
-	uint16_t m_len[XZB_MATCH_LEN_MAX + 1], m_len2[XZB_MATCH_LEN_MAX + 1];
-	uint8_t m_mb[XZB_MATCH_LEN_MAX + 1 + 2];
-	xzb_prob probs[PI_TOTAL + 2];
-	uint8_t prices[128];
-	alignas(8) uint16_t rc_bits[72];   // one symbol's coded bits: probability | bit << 12 | direct << 13 (see rc_run)
-	// ---- helper ("M") warp: state-independent match candidates computed ahead of the DP warp ----
-	MRec mrec[MREC_RING];
-	alignas(16) xzb_pair mring_mp[32][8];
-	uint32_t mring_mh[32];
-	volatile uint32_t m_epoch;      // bumped by the DP warp at every segment start
-	volatile uint32_t m_pos0;       // block position of the segment's cur = 1
-	volatile uint32_t m_position0;  // `position` (pos_state / literal context base) of cur = 1
-	volatile uint32_t m_consumed;   // records of this epoch the DP warp is done with
-	volatile uint32_t m_exit;
-	// ---- fast mode: warp 1 parses ahead (lzma_lzma_optimum_fast needs no coder state), warp 0 codes ----
-	volatile uint64_t f_tag[XZB_FRING];   // (epoch << 32) | (entry number + 1), written last
-	volatile uint32_t f_back[XZB_FRING], f_lenra[XZB_FRING], f_rpos[XZB_FRING];  // back, len | read_ahead << 16, read_pos after the decision
-	volatile uint32_t f_epoch;      // bumped by the coder warp: (re)start parsing at f_start_pos with reps = 0
-	volatile uint32_t f_start_pos;
-	volatile uint32_t f_consumed;   // entries of this epoch the coder warp has taken
-	// ---- back-half ("B") warp mailbox: second half of helper2 runs one position behind the DP warp ----
-	H2 bw_ctx;
-	uint32_t bw_len_in;
-	volatile uint32_t bw_len_end;
-	volatile uint32_t bw_go, bw_done;
-};
-
-struct WSeg { uint32_t base, type, n, v; };  // one run of coded bits of a symbol
-#define SEG_SINGLE 0
-#define SEG_TREE 1
-#define SEG_RTREE 2
-#define SEG_DIRECT 3
-#define SEG_MLIT 4
-
 template <class SM>
 struct WarpEncT {
+	static constexpr bool FAST = SM::FAST;   // fast mode: decisions come from the parser warp, nothing is priced
 	SM &S;
 	const uint32_t lane;
 	// block + match store
@@ -128,12 +59,12 @@ struct WarpEncT {
 	uint32_t read_pos, read_ahead, ring_base;
 	uint32_t f_epoch = 0, f_k = 0;  // coder warp's side of the fast-mode ring
 	// params
-	uint32_t nice_len, fast_mode, pos_mask, lc, literal_mask, dist_table_size, len_table_size, num_pos_states;
+	uint32_t nice_len, pos_mask, lc, literal_mask, dist_table_size, len_table_size, num_pos_states;
 	// coder state (uniform across lanes)
 	uint32_t state, rep0, rep1, rep2, rep3;
 	uint32_t uncomp_size, is_initialized;
 	uint32_t matches_count, longest_match_length;
-	uint32_t match_price_count, align_price_count, opts_end_index, opts_current_index;
+	uint32_t match_price_count, align_price_count;
 	uint32_t n_symbols;
 	// range coder (identical in every lane)
 	uint64_t rc_low; uint32_t rc_cache_size, rc_range, rc_cache, rc_out_pos; uint8_t *rc_out;
@@ -215,23 +146,19 @@ struct WarpEncT {
 		__syncwarp();
 		rc_low = 0; rc_cache_size = 1; rc_range = 0xFFFFFFFFu; rc_cache = 0;
 		state = 0; rep0 = rep1 = rep2 = rep3 = 0;
-		if constexpr (!SM::FAST_ONLY) {
-			if (!fast_mode)
-				for (uint32_t w = 0; w < 2; ++w)
-					for (uint32_t ps = 0; ps < num_pos_states; ++ps) length_update_prices(w, ps);
-		}
+		if constexpr (!FAST)
+			for (uint32_t w = 0; w < 2; ++w)
+				for (uint32_t ps = 0; ps < num_pos_states; ++ps) length_update_prices(w, ps);
 		match_price_count = 0xFFFFFFFFu / 2;
 		align_price_count = 0xFFFFFFFFu / 2;
-		opts_end_index = 0; opts_current_index = 0;
 	}
 
 	// ---------------- match store reader ----------------
 	__device__ __forceinline__ uint32_t mf_avail() const { return size - read_pos; }
 
 	// The binary-tree match finder publishes its progress segment by segment while this kernel runs
-	// (xzb_k_publish).  Only this warp polls; it asks for XZB_MF_MARGIN positions beyond its own refill
-	// so that the helper warp, at most MREC_RING positions and one 32-position refill ahead, never
-	// reads an unfinished row.  Segment boundaries are multiples of 256 positions, so a cache line of
+	// (xzb_k_publish).  Only this warp polls; at a refill it asks for XZB_MF_MARGIN positions beyond
+	// the refill's first position.  Segment boundaries are multiples of 256 positions, so a cache line of
 	// mh/mp never mixes finished and unfinished rows; the overflow pool is read past L1 (__ldcg).
 	__device__ __forceinline__ void mf_wait(uint32_t need)
 	{
@@ -484,60 +411,6 @@ struct WarpEncT {
 		__syncwarp();
 	}
 
-	// Bits of up to 8 segments: each lane resolves the probability index of "its" bit in closed form,
-	// adapts that probability, and the low/range recurrence then consumes the bits in order.
-	__device__ void encode_segments(const WSeg *segs, uint32_t nseg, uint32_t mlit_symbol, uint32_t mlit_match_byte)
-	{
-		uint32_t total = 0;
-		for (uint32_t k = 0; k < nseg; ++k) total += segs[k].n;
-		uint32_t pv[2] = { 0xFFFF, 0xFFFF }, bv[2] = { 0, 0 };
-#pragma unroll
-		for (uint32_t rnd = 0; rnd < 2; ++rnd) {
-			const uint32_t s = lane + 32 * rnd;
-			if (s < total) {
-				uint32_t k = 0, start = 0;
-				while (s >= start + segs[k].n) { start += segs[k].n; ++k; }
-				const uint32_t j = s - start;
-				const WSeg sg = segs[k];
-				uint32_t idx = 0xFFFF, bit;
-				if (sg.type == SEG_SINGLE) { idx = sg.base; bit = sg.v; }
-				else if (sg.type == SEG_TREE) {
-					idx = sg.base + ((1u << j) | (sg.v >> (sg.n - j)));
-					bit = (sg.v >> (sg.n - 1 - j)) & 1;
-				} else if (sg.type == SEG_RTREE) {
-					uint32_t m = 1;
-					for (uint32_t t = 0; t < j; ++t) m = (m << 1) + ((sg.v >> t) & 1);
-					idx = sg.base + m;
-					bit = (sg.v >> j) & 1;
-				} else if (sg.type == SEG_DIRECT) {
-					bit = (sg.v >> (sg.n - 1 - j)) & 1;
-				} else {  // SEG_MLIT: literal coded against a match byte (lzma_encoder.c:22-43)
-					const uint32_t pre = (mlit_symbol | 0x100) >> (8 - j);
-					const uint32_t off = ((mlit_symbol ^ mlit_match_byte) >> (8 - j)) == 0 ? 0x100u : 0u;
-					const uint32_t mbit = ((mlit_match_byte >> (7 - j)) & 1) ? off : 0u;
-					idx = sg.base + off + mbit + pre;
-					bit = (mlit_symbol >> (7 - j)) & 1;
-				}
-				bv[rnd] = bit;
-				if (idx != 0xFFFF) {
-					const uint32_t p = S.probs[idx];
-					pv[rnd] = p;
-					S.probs[idx] = (xzb_prob)(bit ? p - (p >> 5) : p + ((2048 - p) >> 5));
-				}
-			}
-		}
-		// Direct bits (only the middle of a far distance, one contiguous run) are told apart once per
-		// symbol, not once per coded bit: [0, d0) and (d1, n0) are probability bits, [d0, d1] direct bits.
-		const uint32_t n0 = total < 32 ? total : 32;
-		const uint32_t dmask = __ballot_sync(WFULL, lane < n0 && pv[0] == 0xFFFF);
-		const uint32_t d0 = dmask ? (uint32_t)__ffs((int)dmask) - 1 : n0, d1 = dmask ? 31u - (uint32_t)__clz((int)dmask) : n0;
-		for (uint32_t i = 0; i < d0; ++i) rc_step_prob(__shfl_sync(WFULL, pv[0], i), __shfl_sync(WFULL, bv[0], i));
-		for (uint32_t i = d0; i < n0 && i <= d1; ++i) rc_step(__shfl_sync(WFULL, pv[0], i), __shfl_sync(WFULL, bv[0], i));
-		for (uint32_t i = d1 + 1; i < n0; ++i) rc_step_prob(__shfl_sync(WFULL, pv[0], i), __shfl_sync(WFULL, bv[0], i));
-		for (uint32_t i = 32; i < total; ++i) rc_step(__shfl_sync(WFULL, pv[1], i - 32), __shfl_sync(WFULL, bv[1], i - 32));
-		__syncwarp();
-	}
-
 	// ---- one symbol's bits: resolved by the lanes in closed form, coded from a shared-memory list ----
 	// The low/range recurrence (range_encoder.h:196-234) is the only serial part of a symbol.  The lanes
 	// put (probability before adaptation | bit << 12 | direct-bit flag << 13) of "their" bit into
@@ -650,8 +523,7 @@ struct WarpEncT {
 	// from before this length's own bits (DESIGN.md F2)
 	__device__ __forceinline__ void length_count(uint32_t which, uint32_t pos_state)
 	{
-		if constexpr (SM::FAST_ONLY) return;
-		else if (!fast_mode) {
+		if constexpr (!FAST) {
 			const uint32_t c = S.len_counters[which][pos_state] - 1;
 			__syncwarp();
 			if (c == 0) length_update_prices(which, pos_state);
@@ -713,7 +585,7 @@ struct WarpEncT {
 		const uint32_t sub = PI_LITERAL + 3u * ((((position << 8) + buf[p - 1]) & literal_mask) << lc);
 		const bool matched = state >= XZB_LIT_STATES;
 		const uint32_t mb = matched ? buf[p - rep0 - 1] : 0;
-		uint32_t idx = 0, bit = 0, pvv = 0;
+		uint32_t idx = 0, bit = 0;
 		if (lane == 0) {
 			idx = PI_IS_MATCH + (state << 4) + pos_state;
 		} else if (lane < 9) {
@@ -727,41 +599,10 @@ struct WarpEncT {
 				idx = sub + off + mbit + pre;
 			}
 		}
-		(void)pvv;
 		if (lane < 9) rc_put(lane, idx, bit);
 		state = matched ? (state <= 9 ? state - 3 : state - 6) : (state <= 3 ? 0 : state - 3);
 		rc_run(9);
 		read_ahead -= 1;
-	}
-
-	// segments of a length (lzma_encoder.c:105-134); returns number of segments appended
-	__device__ uint32_t length_segments(WSeg *segs, uint32_t which, uint32_t pos_state, uint32_t len)
-	{
-		const uint32_t base = which ? PI_REP_LEN : PI_MATCH_LEN;
-		if (!fast_mode) {
-			// price refresh must see the probabilities from before this length's own bits
-			const uint32_t c = S.len_counters[which][pos_state] - 1;
-			__syncwarp();
-			if (c == 0) length_update_prices(which, pos_state);
-			else { if (lane == 0) S.len_counters[which][pos_state] = c; __syncwarp(); }
-		}
-		len -= XZB_MATCH_LEN_MIN;
-		uint32_t n = 0;
-		if (len < XZB_LEN_LOW) {
-			segs[n++] = WSeg{ base + LC_CHOICE, SEG_SINGLE, 1, 0 };
-			segs[n++] = WSeg{ base + LC_LOW + pos_state * 8, SEG_TREE, 3, len };
-		} else {
-			segs[n++] = WSeg{ base + LC_CHOICE, SEG_SINGLE, 1, 1 };
-			len -= XZB_LEN_LOW;
-			if (len < XZB_LEN_MID) {
-				segs[n++] = WSeg{ base + LC_CHOICE2, SEG_SINGLE, 1, 0 };
-				segs[n++] = WSeg{ base + LC_MID + pos_state * 8, SEG_TREE, 3, len };
-			} else {
-				segs[n++] = WSeg{ base + LC_CHOICE2, SEG_SINGLE, 1, 1 };
-				segs[n++] = WSeg{ base + LC_HIGH, SEG_TREE, 8, len - XZB_LEN_MID };
-			}
-		}
-		return n;
 	}
 
 	// encode_symbol (lzma_encoder.c:232-263): literal (:22-69), match (:152-175), rep_match (:178-229)
@@ -873,563 +714,12 @@ struct WarpEncT {
 	}
 	static __device__ __forceinline__ bool xzb_change_pair_w(uint32_t small_dist, uint32_t big_dist) { return (big_dist >> 7) > small_dist; }
 
-	// ---------------- lzma_lzma_optimum_normal ----------------
-	__device__ __forceinline__ void set_opt(uint32_t at, uint32_t price, uint32_t pos_prev, uint32_t back_prev, uint32_t flags)
-	{
-		S.o_price[at] = price; S.o_pos_prev[at] = (uint16_t)pos_prev; S.o_back_prev[at] = back_prev; S.o_flags[at] = (uint8_t)flags;
-	}
-	// opts[++len_end].price = RC_INFINITY_PRICE up to `upto` (uniform)
-	__device__ __forceinline__ uint32_t extend(uint32_t len_end, uint32_t upto)
-	{
-		if (len_end < upto) {
-			for (uint32_t t = len_end + 1 + lane; t <= upto; t += 32) S.o_price[t] = XZB_INFINITY_PRICE;
-			__syncwarp();
-			len_end = upto;
-		}
-		return len_end;
-	}
-
-	__device__ void backward(uint32_t *len_res, uint32_t *back_res, uint32_t cur)  // :222-263
-	{
-		__syncwarp();
-		if (lane == 0) {
-			uint32_t pos_mem = S.o_pos_prev[cur];
-			uint32_t back_mem = S.o_back_prev[cur];
-			uint32_t c = cur;
-			do {
-				const uint32_t fl = S.o_flags[c];
-				if (fl & 1) {
-					S.o_back_prev[pos_mem] = XZB_BACK_LITERAL; S.o_flags[pos_mem] &= ~1u;
-					S.o_pos_prev[pos_mem] = (uint16_t)(pos_mem - 1);
-					if (fl & 2) {
-						S.o_flags[pos_mem - 1] &= ~1u;
-						S.o_pos_prev[pos_mem - 1] = S.o_pos_prev_2[c];
-						S.o_back_prev[pos_mem - 1] = S.o_back_prev_2[c];
-					}
-				}
-				const uint32_t pos_prev = pos_mem, back_cur = back_mem;
-				back_mem = S.o_back_prev[pos_prev];
-				pos_mem = S.o_pos_prev[pos_prev];
-				S.o_back_prev[pos_prev] = back_cur;
-				S.o_pos_prev[pos_prev] = (uint16_t)c;
-				c = pos_prev;
-			} while (c != 0);
-		}
-		__syncwarp();
-		opts_end_index = cur;
-		opts_current_index = S.o_pos_prev[0];
-		*len_res = S.o_pos_prev[0];
-		*back_res = S.o_back_prev[0];
-	}
-
 	// index of the first match whose len >= l (matches sorted by len); uniform or per-lane
 	__device__ __forceinline__ uint32_t match_index_for(uint32_t l, uint32_t mcount) const
 	{
 		uint32_t i = 0;
 		while (i + 1 < mcount && S.m_len[i] < l) ++i;
 		return i;
-	}
-
-	__device__ uint32_t helper1(uint32_t *back_res, uint32_t *len_res, uint32_t position)  // :270-439
-	{
-		uint32_t len_main, mcount;
-		if (read_ahead == 0) {
-			len_main = mf_find(&mcount);
-		} else {
-			len_main = longest_match_length;
-			mcount = matches_count;
-		}
-		const uint32_t buf_avail = xzb_min(mf_avail() + 1, XZB_MATCH_LEN_MAX);
-		if (buf_avail < 2) { *back_res = XZB_BACK_LITERAL; *len_res = 1; return 0xFFFFFFFFu; }
-		const uint8_t *b = buf + read_pos - 1;
-		uint32_t rl[4];
-		rep_lens4(b, buf_avail, rl);
-		uint32_t rep_max_index = 0;
-		for (uint32_t i = 1; i < XZB_REPS; ++i) if (rl[i] > rl[rep_max_index]) rep_max_index = i;
-		if (rl[rep_max_index] >= nice_len) {
-			*back_res = rep_max_index; *len_res = rl[rep_max_index];
-			mf_skip(*len_res - 1); return 0xFFFFFFFFu;
-		}
-		if (len_main >= nice_len) {
-			*back_res = S.m_dist[mcount - 1] + XZB_REPS; *len_res = len_main;
-			mf_skip(len_main - 1); return 0xFFFFFFFFu;
-		}
-		const uint32_t current_byte = b[0];
-		const uint32_t match_byte = *(b - rep0 - 1);
-		if (len_main < 2 && current_byte != match_byte && rl[rep_max_index] < 2) {
-			*back_res = XZB_BACK_LITERAL; *len_res = 1; return 0xFFFFFFFFu;
-		}
-		const uint32_t pos_state = position & pos_mask;
-		const uint32_t lit = literal_price(position, b[-1], state >= XZB_LIT_STATES, match_byte, current_byte);
-		uint32_t price1 = pr0(PI_IS_MATCH + (state << 4) + pos_state) + lit;
-		uint32_t back1 = XZB_BACK_LITERAL;
-		const uint32_t match_price = pr1(PI_IS_MATCH + (state << 4) + pos_state);
-		const uint32_t rep_match_price = match_price + pr1(PI_IS_REP + state);
-		if (match_byte == current_byte) {
-			const uint32_t srp = rep_match_price + short_rep_price(state, pos_state);
-			if (srp < price1) { price1 = srp; back1 = 0; }
-		}
-		const uint32_t len_end = xzb_max(len_main, rl[rep_max_index]);
-		if (len_end < 2) { *back_res = back1; *len_res = 1; return 0xFFFFFFFFu; }
-		__syncwarp();
-		if (lane == 0) {
-			S.o_state[0] = (uint8_t)state;
-			S.o_backs[0] = make_uint4(rep0, rep1, rep2, rep3);
-			set_opt(1, price1, 0, back1, 0);
-		}
-		for (uint32_t t = 2 + lane; t <= len_end; t += 32) S.o_price[t] = XZB_INFINITY_PRICE;
-		__syncwarp();
-		for (uint32_t i = 0; i < XZB_REPS; ++i) {
-			const uint32_t rep_len = rl[i];
-			if (rep_len < 2) continue;
-			const uint32_t price = rep_match_price + pure_rep_price(i, state, pos_state);
-			for (uint32_t l = 2 + lane; l <= rep_len; l += 32) {
-				const uint32_t p = price + len_price(1, l, pos_state);
-				if (p < S.o_price[l]) set_opt(l, p, 0, i, 0);
-			}
-			__syncwarp();
-		}
-		const uint32_t normal_match_price = match_price + pr0(PI_IS_REP + state);
-		const uint32_t start = rl[0] >= 2 ? rl[0] + 1 : 2;
-		if (start <= len_main) {
-			for (uint32_t l = start + lane; l <= len_main; l += 32) {
-				const uint32_t i = match_index_for(l, mcount);
-				const uint32_t dist = S.m_dist[i];
-				const uint32_t p = normal_match_price + dist_len_price(dist, l, pos_state);
-				if (p < S.o_price[l]) set_opt(l, p, 0, dist + XZB_REPS, 0);
-			}
-			__syncwarp();
-		}
-		return len_end;
-	}
-
-	// "X + literal + rep0" candidate after a rep/match of length len_test ending at cur+len_test
-	// (:635-687 for reps, :729-790 for matches).  price_x = price up to and including X.
-	__device__ uint32_t xlr_candidate(uint32_t price_x, uint32_t state_after_x, const uint8_t *b, const uint8_t *bb, uint32_t len_test,
-			uint32_t position, uint32_t cur, uint32_t back_code, uint32_t len_end, uint32_t buf_avail_full)
-	{
-		uint32_t len_test_2 = len_test + 1;
-		const uint32_t limit = xzb_min(buf_avail_full, len_test_2 + nice_len);
-		if (len_test_2 < limit) len_test_2 = memcmplen(b, bb, len_test_2, limit);
-		len_test_2 -= len_test + 1;
-		if (len_test_2 >= 2) {
-			uint32_t state_2 = state_after_x;
-			uint32_t psn = (position + len_test) & pos_mask;
-			const uint32_t calp = price_x + pr0(PI_IS_MATCH + (state_2 << 4) + psn)
-					+ literal_price(position + len_test, b[len_test - 1], true, bb[len_test], b[len_test]);
-			state_2 = xzb_st_literal_w(state_2);
-			psn = (position + len_test + 1) & pos_mask;
-			const uint32_t nrmp = calp + pr1(PI_IS_MATCH + (state_2 << 4) + psn) + pr1(PI_IS_REP + state_2);
-			const uint32_t offset = cur + len_test + 1 + len_test_2;
-			len_end = extend(len_end, offset);
-			const uint32_t p = nrmp + rep_price(0, len_test_2, state_2, psn);
-			if (p < S.o_price[offset]) {
-				__syncwarp();
-				if (lane == 0) {
-					set_opt(offset, p, cur + len_test + 1, 0, 3);
-					S.o_pos_prev_2[offset] = (uint16_t)cur; S.o_back_prev_2[offset] = back_code;
-				}
-				__syncwarp();
-			}
-		}
-		return len_end;
-	}
-	static __device__ __forceinline__ uint32_t xzb_st_literal_w(uint32_t s) { return s <= 3 ? 0 : (s <= 9 ? s - 3 : s - 6); }
-
-	// ---- helper2 (:442-799) in three parts so that the second half can run on another warp ----
-	// Part 1 (needs opts[cur] final): state / reps of this node, window bytes, literal price.
-	__device__ void h2_front(H2 &c, const uint32_t cur, const uint32_t position, const uint32_t buf_avail_full)
-	{
-		const uint8_t *b = buf + read_pos - 1;
-		c.cur = cur; c.position = position; c.bpos = read_pos - 1; c.buf_avail_full = buf_avail_full;
-		c.mcount = matches_count; c.new_len = longest_match_length;
-		uint32_t pos_prev = S.o_pos_prev[cur];
-		const uint32_t fl = S.o_flags[cur];
-		uint32_t st;
-		if (fl & 1) {
-			--pos_prev;
-			if (fl & 2) {
-				st = S.o_state[S.o_pos_prev_2[cur]];
-				st = S.o_back_prev_2[cur] < XZB_REPS ? (st < XZB_LIT_STATES ? 8u : 11u) : (st < XZB_LIT_STATES ? 7u : 10u);
-			} else {
-				st = S.o_state[pos_prev];
-			}
-			st = xzb_st_literal_w(st);
-		} else {
-			st = S.o_state[pos_prev];
-		}
-		// reps of this node (r0..r3) are carried in registers across positions like the reference's reps[]
-		if (pos_prev == cur - 1) {
-			if (S.o_back_prev[cur] == 0) st = st < XZB_LIT_STATES ? 9u : 11u;
-			else st = xzb_st_literal_w(st);
-		} else {
-			uint32_t pos;
-			if ((fl & 1) && (fl & 2)) {
-				pos_prev = S.o_pos_prev_2[cur];
-				pos = S.o_back_prev_2[cur];
-				st = st < XZB_LIT_STATES ? 8u : 11u;
-			} else {
-				pos = S.o_back_prev[cur];
-				st = pos < XZB_REPS ? (st < XZB_LIT_STATES ? 8u : 11u) : (st < XZB_LIT_STATES ? 7u : 10u);
-			}
-			const uint4 pb = S.o_backs[pos_prev];
-			if (pos < XZB_REPS) {
-				if (pos == 0) { h_r0 = pb.x; h_r1 = pb.y; h_r2 = pb.z; h_r3 = pb.w; }
-				else if (pos == 1) { h_r0 = pb.y; h_r1 = pb.x; h_r2 = pb.z; h_r3 = pb.w; }
-				else if (pos == 2) { h_r0 = pb.z; h_r1 = pb.x; h_r2 = pb.y; h_r3 = pb.w; }
-				else { h_r0 = pb.w; h_r1 = pb.x; h_r2 = pb.y; h_r3 = pb.z; }
-			} else {
-				h_r0 = pos - XZB_REPS; h_r1 = pb.x; h_r2 = pb.y; h_r3 = pb.z;
-			}
-		}
-		__syncwarp();
-		if (lane == 0) { S.o_state[cur] = (uint8_t)st; S.o_backs[cur] = make_uint4(h_r0, h_r1, h_r2, h_r3); }
-		c.st = st; c.hr[0] = h_r0; c.hr[1] = h_r1; c.hr[2] = h_r2; c.hr[3] = h_r3;
-		const uint32_t cur_price = S.o_price[cur];
-		// One round of window loads serves the whole rep phase: lane = (rep index, byte 0..7).
-		const uint32_t buf_avail = xzb_min(buf_avail_full, nice_len);
-		const uint32_t hr[4] = { h_r0, h_r1, h_r2, h_r3 };
-		uint32_t rmask;
-		uint32_t current_byte, match_byte;
-		{
-			const uint32_t j = lane & 7;
-			const uint32_t rr = hr[lane >> 3];
-			const bool in = j < buf_avail;
-			const uint32_t av = in ? b[j] : 0u, cv = in ? (b - rr - 1)[j] : 0x100u;
-			rmask = __ballot_sync(WFULL, av != cv);
-			current_byte = __shfl_sync(WFULL, av, 0);
-			match_byte = __shfl_sync(WFULL, cv, 0);
-		}
-		const uint32_t pos_state = position & pos_mask;
-		const uint32_t lit = literal_price(position, b[-1], st >= XZB_LIT_STATES, match_byte, current_byte);
-		const uint32_t cur_and_1_price = cur_price + pr0(PI_IS_MATCH + (st << 4) + pos_state) + lit;
-		c.cur_price = cur_price; c.buf_avail = buf_avail; c.rmask = rmask; c.current_byte = current_byte; c.match_byte = match_byte;
-		c.pos_state = pos_state; c.cur_and_1_price = cur_and_1_price;
-		c.match_price = cur_price + pr1(PI_IS_MATCH + (st << 4) + pos_state);
-		c.rep_match_price = c.match_price + pr1(PI_IS_REP + st);
-	}
-
-	// Part 2 (needs opts[cur+1] stable): literal / short-rep candidates for cur + 1.
-	__device__ void h2_front_apply(H2 &c)
-	{
-		const uint32_t cur = c.cur, st = c.st, pos_state = c.pos_state, cur_and_1_price = c.cur_and_1_price;
-		const uint32_t match_byte = c.match_byte, current_byte = c.current_byte, rep_match_price = c.rep_match_price;
-		bool next_is_literal = false;
-		uint32_t n_price = S.o_price[cur + 1], n_pos_prev = S.o_pos_prev[cur + 1], n_back_prev = S.o_back_prev[cur + 1];
-		bool n_dirty = false;
-		uint32_t n_flags = S.o_flags[cur + 1];
-		if (cur_and_1_price < n_price) {
-			n_price = cur_and_1_price; n_pos_prev = cur; n_back_prev = XZB_BACK_LITERAL; n_flags = 0; n_dirty = true;
-			next_is_literal = true;
-		}
-		if (match_byte == current_byte && !(n_pos_prev < cur && n_back_prev == 0)) {
-			const uint32_t srp = rep_match_price + short_rep_price(st, pos_state);
-			if (srp <= n_price) {
-				n_price = srp; n_pos_prev = cur; n_back_prev = 0; n_flags = 0; n_dirty = true;
-				next_is_literal = true;
-			}
-		}
-		if (n_dirty) { __syncwarp(); if (lane == 0) set_opt(cur + 1, n_price, n_pos_prev, n_back_prev, n_flags); __syncwarp(); }
-		c.next_is_literal = next_is_literal ? 1u : 0u;
-	}
-
-	// Part 3: literal+rep0, the rep candidates and the match candidates (targets >= cur + 2).
-	__device__ uint32_t h2_back(const H2 &c, uint32_t len_end, const bool mrec_ok)
-	{
-		const uint32_t cur = c.cur, position = c.position, buf_avail_full = c.buf_avail_full, buf_avail = c.buf_avail;
-		const uint32_t st = c.st, rmask = c.rmask, current_byte = c.current_byte, match_byte = c.match_byte, pos_state = c.pos_state;
-		const uint32_t cur_and_1_price = c.cur_and_1_price, match_price = c.match_price, rep_match_price = c.rep_match_price;
-		const bool next_is_literal = c.next_is_literal != 0;
-		const uint32_t h_r0 = c.hr[0];
-		const uint32_t hr[4] = { c.hr[0], c.hr[1], c.hr[2], c.hr[3] };
-		const uint8_t *b = buf + c.bpos;
-		uint32_t mcount = c.mcount, new_len = c.new_len;
-
-		if (!next_is_literal && match_byte != current_byte) {  // literal + rep0, :562-597
-			const uint8_t *bb = b - h_r0 - 1;
-			const uint32_t limit = xzb_min(buf_avail_full, nice_len + 1);
-			const uint32_t len_test = mlen_from(rmask & 0xFF, 1, buf_avail, b, bb, limit) - 1;
-			if (len_test >= 2) {
-				const uint32_t state_2 = xzb_st_literal_w(st);
-				const uint32_t psn = (position + 1) & pos_mask;
-				const uint32_t nrmp = cur_and_1_price + pr1(PI_IS_MATCH + (state_2 << 4) + psn) + pr1(PI_IS_REP + state_2);
-				const uint32_t offset = cur + 1 + len_test;
-				len_end = extend(len_end, offset);
-				const uint32_t p = nrmp + rep_price(0, len_test, state_2, psn);
-				if (p < S.o_price[offset]) {
-					__syncwarp();
-					if (lane == 0) set_opt(offset, p, cur + 1, 0, 1);
-					__syncwarp();
-				}
-			}
-		}
-
-		uint32_t start_len = 2;
-#pragma unroll
-		for (uint32_t rep_index = 0; rep_index < XZB_REPS; ++rep_index) {  // :602-688
-			const uint32_t mg = (rmask >> (8 * rep_index)) & 0xFF;
-			if (mg & 3) continue;  // not_equal_16
-			const uint8_t *bb = b - hr[rep_index] - 1;
-			const uint32_t len_test = mlen_from(mg, 2, buf_avail, b, bb, buf_avail);
-			len_end = extend(len_end, cur + len_test);
-			const uint32_t price = rep_match_price + pure_rep_price(rep_index, st, pos_state);
-			for (uint32_t l = 2 + lane; l <= len_test; l += 32) {
-				const uint32_t p = price + len_price(1, l, pos_state);
-				if (p < S.o_price[cur + l]) set_opt(cur + l, p, cur, rep_index, 0);
-			}
-			__syncwarp();
-			if (rep_index == 0) start_len = len_test + 1;
-			// rep + literal + rep0, :635-687
-			uint32_t len_test_2 = len_test + 1;
-			const uint32_t limit = xzb_min(buf_avail_full, len_test_2 + nice_len);
-			if (len_test_2 < limit) len_test_2 = mlen_from(mg, len_test_2, buf_avail, b, bb, limit);
-			len_test_2 -= len_test + 1;
-			if (len_test_2 >= 2) {
-				uint32_t state_2 = st < XZB_LIT_STATES ? 8u : 11u;
-				uint32_t psn = (position + len_test) & pos_mask;
-				const uint32_t calp = price + len_price(1, len_test, pos_state) + pr0(PI_IS_MATCH + (state_2 << 4) + psn)
-						+ literal_price(position + len_test, b[len_test - 1], true, bb[len_test], b[len_test]);
-				state_2 = xzb_st_literal_w(state_2);
-				psn = (position + len_test + 1) & pos_mask;
-				const uint32_t nrmp = calp + pr1(PI_IS_MATCH + (state_2 << 4) + psn) + pr1(PI_IS_REP + state_2);
-				const uint32_t offset = cur + len_test + 1 + len_test_2;
-				len_end = extend(len_end, offset);
-				const uint32_t p = nrmp + rep_price(0, len_test_2, state_2, psn);
-				if (p < S.o_price[offset]) {
-					__syncwarp();
-					if (lane == 0) {
-						set_opt(offset, p, cur + len_test + 1, 0, 3);
-						S.o_pos_prev_2[offset] = (uint16_t)cur; S.o_back_prev_2[offset] = rep_index;
-					}
-					__syncwarp();
-				}
-			}
-		}
-
-		if (mrec_ok) {
-			// fast path: candidates prepared by the helper warp (see MRec); same application order as below
-			const MRec &R = S.mrec[(cur - 1) % MREC_RING];
-			if (new_len >= start_len) {
-				const uint32_t normal_match_price = match_price + pr0(PI_IS_REP + st);
-				len_end = extend(len_end, cur + new_len);
-				const uint32_t s2 = st < XZB_LIT_STATES ? 7u : 10u;
-				uint32_t off = 0, pp = 0, L = 0, dist = 0;
-				bool valid = false;
-				if (lane < mcount) {
-					L = R.m_len[lane];
-					const uint32_t lt2 = R.m_lt2[lane];
-					if (L >= start_len && lt2 >= 2) {
-						valid = true; dist = R.m_dist[lane];
-						pp = normal_match_price + R.m_rel[lane] + pr0(PI_IS_MATCH + (s2 << 4) + ((position + L) & pos_mask));
-						off = cur + L + 1 + lt2;
-					}
-				}
-				uint32_t todo = __ballot_sync(WFULL, valid);
-				while (todo) {
-					const uint32_t j = (uint32_t)__ffs((int)todo) - 1;
-					todo &= todo - 1;
-					const uint32_t off_j = __shfl_sync(WFULL, off, j), pp_j = __shfl_sync(WFULL, pp, j);
-					len_end = extend(len_end, off_j);
-					if (pp_j < S.o_price[off_j]) {
-						const uint32_t Lj = __shfl_sync(WFULL, L, j), dj = __shfl_sync(WFULL, dist, j);
-						__syncwarp();
-						if (lane == 0) {
-							set_opt(off_j, pp_j, cur + Lj + 1, 0, 3);
-							S.o_pos_prev_2[off_j] = (uint16_t)cur; S.o_back_prev_2[off_j] = dj + XZB_REPS;
-						}
-						__syncwarp();
-					}
-				}
-				for (uint32_t l = start_len + lane; l <= new_len; l += 32) {
-					const uint32_t p = normal_match_price + R.plain_rel[l - 2];
-					if (p < S.o_price[cur + l]) set_opt(cur + l, p, cur, R.m_dist[R.plain_i[l - 2]] + XZB_REPS, 0);
-				}
-				__syncwarp();
-			}
-			return len_end;
-		}
-		if (new_len > buf_avail) {  // :692-700
-			new_len = buf_avail;
-			mcount = 0;
-			while (new_len > S.m_len[mcount]) ++mcount;
-			__syncwarp();
-			if (lane == 0) { S.m_len[mcount] = (uint16_t)new_len; S.m_len2[mcount] = 0x1FF; }  // shortened match: precomputed len2 no longer applies
-			++mcount;
-			__syncwarp();
-		}
-		if (new_len >= start_len) {
-			const uint32_t normal_match_price = match_price + pr0(PI_IS_REP + st);
-			len_end = extend(len_end, cur + new_len);
-			// For one target slot the reference's order is: every "match+literal+rep0" candidate that lands
-			// on it (their match is shorter than the slot's own length), then the plain match candidate.
-			// So: all mlr candidates in match order first, then the plain candidates (one lane per length).
-			for (uint32_t base = 0; base < mcount; base += 32) {
-				const uint32_t i = base + lane;
-				uint32_t off = 0, pp = 0, L = 0, dist = 0;
-				bool valid = false, slow = false;
-				if (i < mcount && S.m_len[i] >= start_len) {
-					L = S.m_len[i]; dist = S.m_dist[i];
-					const uint32_t r = S.m_len2[i];
-					if (r == 0x1FF) {
-						slow = true;
-					} else {
-						uint32_t lt2 = L + 1;
-						const uint32_t limit = xzb_min(buf_avail_full, lt2 + nice_len);
-						if (lt2 < limit) lt2 = xzb_min(L + 1 + r, limit);
-						lt2 -= L + 1;
-						if (lt2 >= 2) {
-							valid = true;
-							const uint32_t price_x = normal_match_price + dist_len_price(dist, L, pos_state);
-							uint32_t state_2 = st < XZB_LIT_STATES ? 7u : 10u;
-							uint32_t psn = (position + L) & pos_mask;
-							const uint32_t calp = price_x + pr0(PI_IS_MATCH + (state_2 << 4) + psn)
-									+ literal_price_matched_lane(position + L, b[L - 1], S.m_mb[i], b[L]);
-							state_2 = xzb_st_literal_w(state_2);
-							psn = (position + L + 1) & pos_mask;
-							const uint32_t nrmp = calp + pr1(PI_IS_MATCH + (state_2 << 4) + psn) + pr1(PI_IS_REP + state_2);
-							off = cur + L + 1 + lt2;
-							pp = nrmp + rep_price(0, lt2, state_2, psn);
-						}
-					}
-				}
-				const uint32_t slow_mask = __ballot_sync(WFULL, slow);
-				uint32_t todo = __ballot_sync(WFULL, valid) | slow_mask;
-				while (todo) {  // in match order
-					const uint32_t j = (uint32_t)__ffs((int)todo) - 1;
-					todo &= todo - 1;
-					if ((slow_mask >> j) & 1) {
-						const uint32_t Lj = S.m_len[base + j], dj = S.m_dist[base + j];
-						len_end = xlr_candidate(normal_match_price + dist_len_price(dj, Lj, pos_state), st < XZB_LIT_STATES ? 7u : 10u, b, b - dj - 1, Lj,
-								position, cur, dj + XZB_REPS, len_end, buf_avail_full);
-					} else {
-						const uint32_t off_j = __shfl_sync(WFULL, off, j), pp_j = __shfl_sync(WFULL, pp, j);
-						len_end = extend(len_end, off_j);
-						if (pp_j < S.o_price[off_j]) {
-							const uint32_t Lj = __shfl_sync(WFULL, L, j), dj = __shfl_sync(WFULL, dist, j);
-							__syncwarp();
-							if (lane == 0) {
-								set_opt(off_j, pp_j, cur + Lj + 1, 0, 3);
-								S.o_pos_prev_2[off_j] = (uint16_t)cur; S.o_back_prev_2[off_j] = dj + XZB_REPS;
-							}
-							__syncwarp();
-						}
-					}
-				}
-			}
-			for (uint32_t l = start_len + lane; l <= new_len; l += 32) {
-				const uint32_t i = match_index_for(l, mcount);
-				const uint32_t cur_back = S.m_dist[i];
-				const uint32_t p = normal_match_price + dist_len_price(cur_back, l, pos_state);
-				if (p < S.o_price[cur + l]) set_opt(cur + l, p, cur, cur_back + XZB_REPS, 0);
-			}
-			__syncwarp();
-		}
-		return len_end;
-	}
-
-	__device__ uint32_t helper2(uint32_t len_end, uint32_t position, const uint32_t cur, const uint32_t buf_avail_full, const bool mrec_ok)
-	{
-		H2 c;
-		h2_front(c, cur, position, buf_avail_full);
-		h2_front_apply(c);
-		if (buf_avail_full < 2) return len_end;
-		return h2_back(c, len_end, mrec_ok);
-	}
-	uint32_t h_r0, h_r1, h_r2, h_r3;  // reps[] of lzma_lzma_optimum_normal, carried across helper2 calls
-	bool use_mwarp;
-	uint32_t bw_posted;  // sequence number of the last position handed to the B warp
-
-	// Wait until the B warp has finished the position it was given; pick up its len_end.
-	__device__ __forceinline__ void sync_b(bool &b_out, uint32_t b_cur, uint32_t &len_end)
-	{
-		if (!b_out) return;
-		while (S.bw_done != bw_posted) { }
-		__threadfence_block();
-		len_end = S.bw_len_end;
-		__syncwarp();
-		if (lane == 0) S.m_consumed = b_cur;
-		b_out = false;
-	}
-
-	__device__ void optimum_normal(uint32_t *back_res, uint32_t *len_res, uint32_t position)  // :802-858
-	{
-		if (opts_end_index != opts_current_index) {
-			const uint32_t nxt = S.o_pos_prev[opts_current_index];
-			*len_res = nxt - opts_current_index;
-			*back_res = S.o_back_prev[opts_current_index];
-			opts_current_index = nxt;
-			return;
-		}
-		if (read_ahead == 0) {
-			if (match_price_count >= (1 << 7)) fill_dist_prices();
-			if (align_price_count >= XZB_ALIGN_SIZE) fill_align_prices();
-		}
-		uint32_t len_end = helper1(back_res, len_res, position);
-		if (len_end == 0xFFFFFFFFu) return;
-		h_r0 = rep0; h_r1 = rep1; h_r2 = rep2; h_r3 = rep3;
-		// start the helper warp on this segment: positions read_pos, read_pos+1, ... (cur = 1, 2, ...)
-		const uint32_t epoch = (S.m_epoch + 1) & 0x7FFF;
-		if (use_mwarp) {
-			__syncwarp();
-			if (lane < MREC_RING) S.mrec[lane].tag = 0;
-			__syncwarp();
-			if (lane == 0) {
-				S.m_pos0 = read_pos; S.m_position0 = position + 1; S.m_consumed = 0;
-				__threadfence_block();
-				S.m_epoch = epoch;
-			}
-			__syncwarp();
-		}
-		// Pipelined DP: this warp does part 1/2 of position cur while the B warp still runs part 3 of
-		// position cur - 1 (whose candidates all land at >= cur + 1, never on opts[cur]).
-		uint32_t cur;
-		bool b_out = false;
-		uint32_t b_cur = 0;
-		for (cur = 1;; ++cur) {
-			if (cur >= len_end) {
-				sync_b(b_out, b_cur, len_end);
-				if (cur >= len_end) break;
-			}
-			bool mrec_ok = false;
-			if (use_mwarp && cur <= 0xFFFF) {
-				// the helper warp's record carries count / longest; the match list itself is only needed
-				// on the rare slow paths and when the segment stops here (helper1 of the next call reuses it)
-				const volatile MRec *R = &S.mrec[(cur - 1) % MREC_RING];
-				const uint32_t want = ((epoch << 16) | (cur - 1)) + 1;
-				while (R->tag != want) { }
-				__threadfence_block();
-				matches_count = R->count; longest_match_length = R->longest;
-				mrec_ok = R->slow == 0 && cur + 600 < XZB_OPTS;
-				if (!mrec_ok || longest_match_length >= nice_len) { sync_b(b_out, b_cur, len_end); mf_load(read_pos); }
-				++read_pos; ++read_ahead;
-			} else {
-				longest_match_length = mf_find(&matches_count);
-			}
-			if (longest_match_length >= nice_len) break;
-			const uint32_t baf = xzb_min(mf_avail() + 1, XZB_OPTS - 1 - cur);
-			if (!mrec_ok) {
-				sync_b(b_out, b_cur, len_end);
-				len_end = helper2(len_end, position + cur, cur, baf, false);
-				if (use_mwarp) { __syncwarp(); if (lane == 0) S.m_consumed = cur; }
-				continue;
-			}
-			H2 c;
-			h2_front(c, cur, position + cur, baf);
-			sync_b(b_out, b_cur, len_end);  // part 3 of cur - 1 is complete: opts[cur + 1] is stable now
-			h2_front_apply(c);
-			if (baf < 2) { __syncwarp(); if (lane == 0) S.m_consumed = cur; continue; }
-			__syncwarp();
-			if (lane == 0) {
-				S.bw_ctx = c; S.bw_len_in = len_end;
-				__threadfence_block();
-				S.bw_go = ++bw_posted;
-			} else {
-				++bw_posted;
-			}
-			b_out = true; b_cur = cur;
-		}
-		sync_b(b_out, b_cur, len_end);
-		backward(len_res, back_res, cur);
 	}
 
 	// ---------------- fast mode: decisions come from the parser warp (xzb_w_fast_parser_main) ----------------
@@ -1460,7 +750,8 @@ struct WarpEncT {
 		__syncwarp();
 	}
 
-	// ---------------- lzma_lzma_encode for one LZMA2 chunk (lzma_encoder.c:266-436) ----------------
+	// ---------------- lzma_lzma_encode for one LZMA2 chunk (lzma_encoder.c:266-436), fast mode ----------------
+	// (normal mode: DpEnc::encode_chunk)
 	__device__ void encode_chunk(uint32_t limit)
 	{
 		if (!is_initialized) {
@@ -1477,7 +768,7 @@ struct WarpEncT {
 				++uncomp_size;
 			}
 			is_initialized = 1;
-			if (fast_mode) fast_restart(read_pos);
+			fast_restart(read_pos);
 		}
 		for (;;) {
 			if (read_pos - read_ahead >= limit || rc_pending_reaches(XZB_LZMA2_CHUNK_MAX - XZB_LOOP_INPUT_MAX)) break;
@@ -1485,22 +776,14 @@ struct WarpEncT {
 			if (mf_stalled) break;
 			if constexpr (SM::RCQ != 0) { while (rq_head - S.rcq_tail > SM::RCQ - 128u) { } }   // ring space for one symbol
 			uint32_t len, back;
-			if constexpr (SM::FAST_ONLY) {
-				fast_pop(&back, &len);
-				if (back == XZB_BACK_STALL) { mf_stalled = true; break; }
-			} else if (fast_mode) {
-				fast_pop(&back, &len);
-				if (back == XZB_BACK_STALL) { mf_stalled = true; break; }
-			} else {
-				optimum_normal(&back, &len, uncomp_size);
-			}
+			fast_pop(&back, &len);
+			if (back == XZB_BACK_STALL) { mf_stalled = true; break; }
 			encode_symbol(back, len, uncomp_size);
 			uncomp_size += len;
 		}
 		rc_flush();
 	}
 };
-typedef WarpEncT<WS> WarpEnc;
 
 // Fast mode (presets 0-3), warp 1: lzma_lzma_optimum_fast (lzma_encoder_optimum_fast.c:19-169) looks only at
 // the match store, the window and the four reps -- never at probabilities or the range coder -- so the
@@ -1599,123 +882,27 @@ __device__ inline void xzb_w_coder_main(SM &S, ENC &H)
 }
 
 // Shared memory of the fast-mode kernel xzb_k_parse_fast (presets 0-3): lzma_lzma_optimum_fast needs no price table
-// and no opts[] array, so a Block's coder state is 36 KB and several Blocks share an SM.
+// and no opts[] array, so a Block's coder state is 38 KB.  CODER_WARP: the range coder's arithmetic runs on a warp
+// of its own (xzb_w_coder_main), fed through rcq; otherwise the coding warp runs it and rcq stays unused.
+template <bool CODER_WARP>
 struct FS {
-	static constexpr uint32_t RCQ = 2048;
-	static constexpr bool FAST_ONLY = true;
+	static constexpr uint32_t RCQ_SIZE = 2048;
+	static constexpr uint32_t RCQ = CODER_WARP ? RCQ_SIZE : 0u;
+	static constexpr bool FAST = true;
 	alignas(16) xzb_pair ring_mp[32][8];
 	uint32_t ring_mh[32];
 	uint32_t m_dist[XZB_MATCH_LEN_MAX + 1];
 	uint16_t m_len[XZB_MATCH_LEN_MAX + 1], m_len2[XZB_MATCH_LEN_MAX + 1];
 	uint8_t m_mb[XZB_MATCH_LEN_MAX + 1 + 2];
 	xzb_prob probs[PI_TOTAL + 2];
-	uint8_t prices[128];
 	alignas(8) uint16_t rc_bits[72];
 	volatile uint64_t f_tag[XZB_FRING];
 	volatile uint32_t f_back[XZB_FRING], f_lenra[XZB_FRING], f_rpos[XZB_FRING];
 	volatile uint32_t f_epoch, f_start_pos, f_consumed, m_exit;
-	alignas(4) uint16_t rcq[RCQ];
+	alignas(4) uint16_t rcq[RCQ_SIZE];
 	uint8_t *rcq_out;
 	volatile uint32_t rcq_head, rcq_tail, rcq_T, rcq_flushes, rcq_out_pos;
 };
-
-// Helper warp: for the segment announced by the DP warp, produce MRec records for cur = 1, 2, ...
-// (at most MREC_RING ahead).  Reads probabilities / price tables, which are frozen while a
-// segment's DP runs; records of an abandoned segment are simply never consumed.
-__device__ inline void xzb_w_helper_main(WS &S, WarpEnc &H)
-{
-	const uint32_t lane = H.lane;
-	uint32_t my_epoch = 0;
-	uint32_t ring_base = 0x80000000u;
-	for (;;) {
-		uint32_t e;
-		while ((e = S.m_epoch) == my_epoch) { if (S.m_exit) return; __nanosleep(40); }
-		__threadfence_block();
-		my_epoch = e;
-		const uint32_t pos0 = S.m_pos0, position0 = S.m_position0;
-		for (uint32_t k = 0; k < 0xFFFF; ++k) {
-			while (k >= S.m_consumed + MREC_RING && S.m_epoch == my_epoch && !S.m_exit) __nanosleep(40);
-			if (S.m_epoch != my_epoch || S.m_exit) break;
-			const uint32_t p = pos0 + k;
-			if (p >= H.size) break;
-			const uint32_t position = position0 + k;
-			const uint32_t ps = position & H.pos_mask;
-			if (p - ring_base >= 32u) {  // refill the helper's own view of the match store
-				__syncwarp();
-				ring_base = p;
-				const uint32_t g = p + lane;
-				if (g < H.size) {
-					S.mring_mh[lane] = H.g_mh[g];
-					const uint4 *src = reinterpret_cast<const uint4 *>(H.g_mp + (size_t)g * 8);
-					uint4 *dst = reinterpret_cast<uint4 *>(&S.mring_mp[lane][0]);
-					const uint4 a = src[0], b = src[1], c = src[2], d = src[3];
-					dst[0] = a; dst[1] = b; dst[2] = c; dst[3] = d;
-				}
-				__syncwarp();
-			}
-			const uint32_t slot = p - ring_base;
-			const uint32_t h = S.mring_mh[slot];
-			const uint32_t count = h & 0xFFFF, longest = h >> 16;
-			MRec &R = S.mrec[k % MREC_RING];
-			const bool slow = count > 8;
-			uint32_t L = 0, dist = 0;
-			if (!slow) {
-				const uint8_t *b = H.buf + p;
-				uint32_t lt2 = 0, rel = 0;
-				if (lane < count) {
-					const xzb_pair pr = S.mring_mp[slot][lane];
-					L = XZB_PAIR_LEN(pr.len); dist = pr.dist;
-					const uint32_t r = XZB_PAIR_LEN2(pr.len), mb = XZB_PAIR_MB(pr.len);
-					const uint32_t avail1 = H.size - p;
-					const uint32_t limit = xzb_min(avail1, L + 1 + H.nice_len);
-					if (L + 1 < limit) lt2 = xzb_min(L + 1 + r, limit) - (L + 1);
-					if (lt2 >= 2) {
-						const uint32_t psn2 = (position + L + 1) & H.pos_mask;
-						rel = H.dist_len_price(dist, L, ps) + H.literal_price_matched_lane(position + L, b[L - 1], mb, b[L])
-								+ H.pr1(PI_IS_MATCH + (4u << 4) + psn2) + H.pr1(PI_IS_REP + 4u) + H.rep_price(0, lt2, 4u, psn2);
-					} else {
-						lt2 = 0;
-					}
-					R.m_len[lane] = (uint16_t)L; R.m_lt2[lane] = (uint16_t)lt2; R.m_dist[lane] = dist; R.m_rel[lane] = rel;
-				}
-				const uint32_t nplain = count ? __shfl_sync(WFULL, L, count - 1) : 0;
-				for (uint32_t l = 2 + lane; l - lane <= nplain; l += 32) {  // uniform trip count: shuffles inside
-					uint32_t idx = 0;
-					for (uint32_t j = 0; j + 1 < count; ++j) { const uint32_t Lj = __shfl_sync(WFULL, L, j); if (Lj < l) idx = j + 1; }
-					const uint32_t di = __shfl_sync(WFULL, dist, idx & 31);
-					if (l <= nplain) { R.plain_rel[l - 2] = H.dist_len_price(di, l, ps); R.plain_i[l - 2] = (uint8_t)idx; }
-				}
-				if (lane == 0) R.nplain = (uint16_t)nplain;
-			}
-			if (lane == 0) { R.count = (uint16_t)count; R.longest = (uint16_t)longest; R.slow = slow ? 1 : 0; }
-			__syncwarp();
-			__threadfence_block();
-			if (lane == 0) R.tag = ((my_epoch << 16) | k) + 1;
-			if (longest >= H.nice_len) break;  // the DP loop stops at this position
-		}
-	}
-}
-
-// B warp: part 3 of helper2 (literal+rep0, rep and match candidates) for the position posted by the DP warp.
-__device__ inline void xzb_w_back_main(WS &S, WarpEnc &Bw)
-{
-	uint32_t last = 0;
-	for (;;) {
-		uint32_t g;
-		while ((g = S.bw_go) == last) { if (S.m_exit) return; }
-		__threadfence_block();
-		last = g;
-		const H2 c = S.bw_ctx;
-		uint32_t le = S.bw_len_in;
-		le = Bw.h2_back(c, le, true);
-		__syncwarp();
-		if (Bw.lane == 0) {
-			S.bw_len_end = le;
-			__threadfence_block();
-			S.bw_done = g;
-		}
-	}
-}
 
 struct XzbEncJob;
 
@@ -1748,7 +935,7 @@ __device__ inline int xzb_w_lzma2_encode_block(ENC &E, const XzbParams &P, uint8
 			++*n_chunks_raw;
 			uncompressed_size += E.read_ahead;
 			E.read_ahead = 0;
-			if (E.fast_mode) E.fast_restart(E.read_pos);
+			if constexpr (ENC::FAST) E.fast_restart(E.read_pos);
 			if (E.lane == 0) {
 				out[out_pos] = need_dictionary_reset ? 1 : 2;
 				out[out_pos + 1] = (uint8_t)((uncompressed_size - 1) >> 8);
