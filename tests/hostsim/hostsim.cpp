@@ -170,3 +170,53 @@ extern "C" void hostsim_filter_apply(uint32_t id, uint32_t arg, int enc, uint8_t
 {
 	xzb_filter_apply_seq(XzbPreFilter{ id, arg }, buf, size, enc != 0);
 }
+
+// The container read side (xzb_frame.cuh), each entry point with its results flattened into integers.
+extern "C" {
+
+int hs_stream_header_decode(const uint8_t *in, uint32_t *check)
+{
+	tabs();
+	return xzb_stream_header_decode(g_tab.crc32, in, check);
+}
+
+int hs_stream_footer_decode(const uint8_t *in, uint32_t *check, uint64_t *index_size)
+{
+	tabs();
+	return xzb_stream_footer_decode(g_tab.crc32, in, check, index_size);
+}
+
+// out: hsize, flags, comp (value, end, status), uncomp (value, end, status)
+int hs_block_framing(const uint8_t *h, uint64_t avail, uint64_t out[8])
+{
+	XzbBlockFraming f;
+	if (!xzb_block_framing(h, avail, &f)) return 0;
+	const uint64_t v[8] = { f.hsize, f.flags, f.comp.v, f.comp.end, (uint64_t)f.comp.st, f.uncomp.v, f.uncomp.end, (uint64_t)f.uncomp.st };
+	memcpy(out, v, sizeof(v));
+	return 1;
+}
+
+// out: hsize, comp, uncomp, dict_size, n_pre, then (id, arg) of each filter in front of LZMA2
+int hs_block_header_decode(const uint8_t *h, uint64_t avail, uint64_t out[11])
+{
+	tabs();
+	XzbBlockHeader hb;
+	const int r = xzb_block_header_decode(g_tab.crc32, h, avail, &hb);
+	if (r != XZB_OK) return r;
+	out[0] = hb.hsize; out[1] = hb.comp; out[2] = hb.uncomp; out[3] = hb.dict_size; out[4] = hb.n_pre;
+	for (uint32_t i = 0; i < hb.n_pre; ++i) { out[5 + 2 * i] = hb.pre[i].id; out[6 + 2 * i] = hb.pre[i].arg; }
+	return r;
+}
+
+// want == NULL: nothing to compare against.  out: count, listed, end, stop
+int hs_index_read(const uint8_t *in, uint64_t size, const xzb_index_record *want, uint64_t n_want, uint64_t out[4])
+{
+	tabs();
+	const XzbIndexWant w{ want, n_want };
+	XzbIndexRead x;
+	const int r = xzb_index_read(g_tab.crc32, in, size, want != nullptr ? &w : nullptr, &x);
+	out[0] = x.count; out[1] = x.listed; out[2] = x.end; out[3] = x.stop;
+	return r;
+}
+
+}  // extern "C"

@@ -1,9 +1,13 @@
-// xzb_frame.cuh -- .xz container framing around the LZMA2 payload of one block, plus the
-// Stream Header / Index / Stream Footer.  Host/device.  Reference: common/block_header_encoder.c,
-// common/block_encoder.c:104-133, common/block_buffer_encoder.c:27-162, common/vli_encoder.c,
-// common/index_encoder.c:43-165, common/stream_flags_encoder.c:29-85.
+// xzb_frame.cuh -- the .xz container: framing around the LZMA2 payload of one block, plus the
+// Stream Header / Index / Stream Footer, written (host/device) and read back (host only, at the end).
+// Reference: common/block_header_encoder.c, common/block_encoder.c:104-133,
+// common/block_buffer_encoder.c:27-162, common/vli_encoder.c, common/index_encoder.c:43-165,
+// common/stream_flags_encoder.c:29-85; the read side: common/vli_decoder.c,
+// common/block_header_decoder.c, common/index_hash.c, common/stream_flags_decoder.c.
 #pragma once
 #include "xzb_common.cuh"
+#include "xzb_filters.cuh"
+#include "../../include/xzb200.h"
 
 XZB_HD uint32_t xzb_vli_put(uint8_t *out, uint64_t v)  // vli_encoder.c:16-69 (single call)
 {
@@ -167,4 +171,154 @@ XZB_HD void xzb_block_finish_raw(const uint32_t *crc32_table, const uint8_t *in,
 		res->unpadded_size = (uint64_t)hs + comp + csize;
 		res->fallback = 1;
 	}
+}
+
+// ---- read side (host only), over untrusted input: every reader stays inside the `size` / `avail` bytes it is given ----
+static inline uint32_t xzb_check_field_size(uint32_t check)  // any of the 16 Check IDs, supported or not (check.c:62-86)
+{
+	static const uint8_t sizes[16] = { 0, 4, 4, 4, 8, 8, 8, 16, 16, 16, 32, 32, 32, 64, 64, 64 };
+	return check > 15 ? 0xFFFFFFFFu : sizes[check];
+}
+
+static inline uint32_t xzb_rd32(const uint8_t *p) { return p[0] | ((uint32_t)p[1] << 8) | ((uint32_t)p[2] << 16) | ((uint32_t)p[3] << 24); }
+
+// lzma_vli_decode (single call), vli_decoder.c:16-86.  Whatever the result, *v has the bits read so far and *pos is past
+// the last byte read, so that a lax reader can still use what a strict one rejects.  LONG and NONMIN are invalid.
+enum { XZB_VLI_OK, XZB_VLI_SHORT /* input ran out */, XZB_VLI_LONG /* no last byte in nine */, XZB_VLI_NONMIN /* last byte 0x00 */ };
+static inline int xzb_vli_get(const uint8_t *in, uint64_t *pos, uint64_t size, uint64_t *v)
+{
+	*v = 0;
+	for (uint32_t i = 0; i < 9; ++i) {
+		if (*pos >= size) return XZB_VLI_SHORT;
+		const uint8_t b = in[(*pos)++];
+		*v |= (uint64_t)(b & 0x7F) << (7 * i);
+		if ((b & 0x80) == 0) return (b == 0x00 && i != 0) ? XZB_VLI_NONMIN : XZB_VLI_OK;
+	}
+	return XZB_VLI_LONG;
+}
+static inline int xzb_vli_verdict(int st) { return st == XZB_VLI_OK ? XZB_OK : st == XZB_VLI_SHORT ? XZB_BUF_ERROR : XZB_DATA_ERROR; }
+
+// Stream Header / Footer, stream_flags_decoder.c:26-83, with the verdicts in the reference's order.  Comparing the
+// footer's Index size and Check ID with the Index and the Stream Header is the caller's.
+static inline int xzb_stream_header_decode(const uint32_t *crc32_table, const uint8_t in[12], uint32_t *check)
+{
+	static const uint8_t magic[6] = { 0xFD, 0x37, 0x7A, 0x58, 0x5A, 0x00 };
+	for (int i = 0; i < 6; ++i) if (in[i] != magic[i]) return XZB_FORMAT_ERROR;
+	if (xzb_crc32_bytes(crc32_table, in + 6, 2, 0) != xzb_rd32(in + 8)) return XZB_DATA_ERROR;
+	if (in[6] != 0x00 || (in[7] & 0xF0)) return XZB_OPTIONS_ERROR;
+	*check = in[7] & 0x0F;
+	return XZB_OK;
+}
+static inline int xzb_stream_footer_decode(const uint32_t *crc32_table, const uint8_t in[12], uint32_t *check, uint64_t *index_size)
+{
+	if (in[10] != 'Y' || in[11] != 'Z' || xzb_crc32_bytes(crc32_table, in + 4, 6, 0) != xzb_rd32(in)) return XZB_DATA_ERROR;
+	if (in[8] != 0x00 || (in[9] & 0xF0)) return XZB_OPTIONS_ERROR;
+	*check = in[9] & 0x0F;
+	*index_size = ((uint64_t)xzb_rd32(in + 4) + 1) * 4;  // Backward Size
+	return XZB_OK;
+}
+
+// Block Header framing only (block_header_decoder.c:17-73): Header Size, flags, and the sizes the flags announce, read
+// inside the whole header (CRC32 included), each with its bits so far, its end offset and its xzb_vli_get result; an
+// absent one is 0, zero bytes long, OK.  No CRC32 or filter checks.  False when the header is not all in `avail`.
+struct XzbVliField { uint64_t v; uint32_t end; int st; };
+struct XzbBlockFraming { uint32_t hsize; uint8_t flags; XzbVliField comp, uncomp; };
+static inline bool xzb_block_framing(const uint8_t *h, uint64_t avail, XzbBlockFraming *f)
+{
+	f->hsize = ((uint32_t)h[0] + 1) * 4;
+	if (avail < f->hsize) return false;
+	f->flags = h[1];
+	uint64_t pos = 2;
+	f->comp = XzbVliField{ 0, 2, XZB_VLI_OK };
+	if (f->flags & 0x40) { f->comp.st = xzb_vli_get(h, &pos, f->hsize, &f->comp.v); f->comp.end = (uint32_t)pos; }
+	f->uncomp = XzbVliField{ 0, (uint32_t)pos, XZB_VLI_OK };
+	if (f->flags & 0x80) { f->uncomp.st = xzb_vli_get(h, &pos, f->hsize, &f->uncomp.v); f->uncomp.end = (uint32_t)pos; }
+	return true;
+}
+
+// The full Block Header parse, block_header_decoder.c:17-124 (XZB_BUF_ERROR: not all in `avail`): LZMA2 last, up to
+// three Delta / BCJ filters in front of it.
+struct XzbBlockHeader {
+	uint64_t hsize, comp, uncomp;  // comp/uncomp = UINT64_MAX when absent
+	uint32_t dict_size;
+	uint32_t n_pre;                // filters in front of LZMA2, in chain (= encoding) order
+	XzbPreFilter pre[3];
+};
+static inline int xzb_block_header_decode(const uint32_t *crc32_table, const uint8_t *h, uint64_t avail, XzbBlockHeader *hb)
+{
+	XzbBlockFraming f;
+	if (!xzb_block_framing(h, avail, &f)) return XZB_BUF_ERROR;
+	const uint64_t hin = f.hsize - 4;
+	if (xzb_crc32_bytes(crc32_table, h, (uint32_t)hin, 0) != xzb_rd32(h + hin)) return XZB_DATA_ERROR;
+	if (f.flags & 0x3C) return XZB_OPTIONS_ERROR;
+	if (f.comp.st != XZB_VLI_OK || f.uncomp.st != XZB_VLI_OK || f.uncomp.end > hin) return XZB_DATA_ERROR;  // uncomp.end >= comp.end
+	hb->comp = (f.flags & 0x40) ? f.comp.v : UINT64_MAX;
+	hb->uncomp = (f.flags & 0x80) ? f.uncomp.v : UINT64_MAX;
+	if (hb->comp == 0 || (hb->comp != UINT64_MAX && hb->comp > (UINT64_MAX / 2 - 1024 - 64 - 4))) return XZB_DATA_ERROR;
+	uint64_t hp = f.uncomp.end;
+	const uint32_t nfilters = (f.flags & 3) + 1;
+	bool have = false;
+	hb->n_pre = 0;
+	for (uint32_t i = 0; i < nfilters; ++i) {  // lzma_filter_flags_decode, filter_flags_decoder.c:16-45
+		uint64_t id, psize;
+		if (xzb_vli_get(h, &hp, hin, &id) != XZB_VLI_OK || id >= (1ull << 62)) return XZB_DATA_ERROR;
+		if (xzb_vli_get(h, &hp, hin, &psize) != XZB_VLI_OK || hin - hp < psize) return XZB_DATA_ERROR;
+		if (i + 1 < nfilters) {
+			// a filter in front of the last one: Delta or BCJ (LZMA2 may only be last, validate_chain, filter_common.c:122-249)
+			if (id > 0xFF || !xzb_filter_known((uint32_t)id)) return XZB_OPTIONS_ERROR;
+			XzbPreFilter &pf = hb->pre[hb->n_pre++];
+			pf.id = (uint32_t)id; pf.arg = 0;
+			if (id == XZB_FILTER_DELTA) {          // lzma_delta_props_decode, delta_decoder.c:66-87
+				if (psize != 1) return XZB_OPTIONS_ERROR;
+				pf.arg = (uint32_t)h[hp] + 1;
+			} else {                               // lzma_simple_props_decode, simple_decoder.c:15-39
+				if (psize == 4) pf.arg = xzb_rd32(h + hp);
+				else if (psize != 0) return XZB_OPTIONS_ERROR;
+				if (pf.arg & (xzb_filter_alignment(pf.id) - 1)) return XZB_OPTIONS_ERROR;
+			}
+			hp += psize;
+			continue;
+		}
+		if (id != XZB_FILTER_LZMA2) return XZB_OPTIONS_ERROR;
+		if (psize != 1 || (h[hp] & 0xC0) || h[hp] > 40) return XZB_OPTIONS_ERROR;  // lzma_lzma2_props_decode, lzma2_decoder.c:298-331
+		hb->dict_size = h[hp] == 40 ? 0xFFFFFFFFu : (2u | (h[hp] & 1u)) << (h[hp] / 2u + 11);
+		hp += psize; have = true;
+	}
+	while (hp < hin) if (h[hp++] != 0x00) return XZB_OPTIONS_ERROR;
+	if (!have) return XZB_OPTIONS_ERROR;
+	hb->hsize = f.hsize;
+	return XZB_OK;
+}
+
+// Index, index_hash.c:175-341, from its Indicator at in[0].  The records are walked to their end whatever their VLIs
+// hold, so that a lax reader learns where the Index ends; the verdict is the first fault in stream order, a count or
+// record that differs from *want (when given) included.
+struct XzbIndexWant { const xzb_index_record *recs; uint64_t n; };
+struct XzbIndexRead {
+	uint64_t count;  // Number of Records as stored
+	bool listed;     // false: the input ran out within the records
+	uint64_t end;    // when listed: just past the CRC32 (the records rounded up to four bytes, + 4)
+	uint64_t stop;   // where a strict reader stops: just past the first fault, else = end
+};
+static inline int xzb_index_read(const uint32_t *crc32_table, const uint8_t *in, uint64_t size, const XzbIndexWant *want, XzbIndexRead *x)
+{
+	uint64_t pos = 1, u = 0, w = 0;
+	int ret = XZB_OK, st;
+	auto fault = [&](int verdict) { if (ret == XZB_OK && verdict != XZB_OK) { ret = verdict; x->stop = pos; } };
+	fault(xzb_vli_verdict(st = xzb_vli_get(in, &pos, size, &x->count)));
+	if (want != nullptr && x->count != want->n) fault(XZB_DATA_ERROR);
+	for (uint64_t r = 0; st != XZB_VLI_SHORT && r < x->count; ++r) {
+		fault(xzb_vli_verdict(st = xzb_vli_get(in, &pos, size, &u)));
+		if (st != XZB_VLI_SHORT) fault(xzb_vli_verdict(st = xzb_vli_get(in, &pos, size, &w)));
+		if (ret == XZB_OK && want != nullptr && (u != want->recs[r].unpadded_size || w != want->recs[r].uncompressed_size)) fault(XZB_DATA_ERROR);
+	}
+	x->listed = st != XZB_VLI_SHORT;
+	x->end = ((pos + 3) & ~(uint64_t)3) + 4;
+	while (ret == XZB_OK && (pos & 3)) fault(pos >= size ? XZB_BUF_ERROR : in[pos++] != 0x00 ? XZB_DATA_ERROR : XZB_OK);
+	if (size - pos < 4) fault(XZB_BUF_ERROR);
+	if (ret != XZB_OK) return ret;
+	uint32_t crc = 0xFFFFFFFFu;  // xzb_crc32_bytes for a 64-bit length
+	for (uint64_t i = 0; i < pos; ++i) crc = crc32_table[(crc ^ in[i]) & 0xFF] ^ (crc >> 8);
+	x->stop = pos + 4;
+	return ~crc != xzb_rd32(in + pos) ? XZB_DATA_ERROR : XZB_OK;
 }

@@ -1216,15 +1216,8 @@ extern "C" int xzb_stream_buffer_encode(xzb_ctx *ctx, const uint8_t *in, uint64_
 // ------------------------------------------------------------------------------------
 // Decode
 // ------------------------------------------------------------------------------------
-struct HostBlock {
-	uint64_t hdr_off, hsize, comp, uncomp;  // comp/uncomp = UINT64_MAX when absent
-	uint32_t dict_size;
-	uint32_t n_pre;                         // filters in front of LZMA2, in chain (= encoding) order
-	XzbPreFilter pre[3];
-};
-
 static int decode_batch(xzb_ctx *ctx, const std::vector<XzbDecJob> &jobs, uint32_t check, std::vector<XzbDecResult> &results, std::vector<uint64_t> &crcs,
-		std::vector<uint8_t> *shas = nullptr, const std::vector<HostBlock> *chains = nullptr)
+		std::vector<uint8_t> *shas = nullptr, const std::vector<XzbBlockHeader> *chains = nullptr)
 {
 	cudaStream_t st = ctx->stream;
 	const uint32_t B = (uint32_t)jobs.size();
@@ -1249,11 +1242,11 @@ static int decode_batch(xzb_ctx *ctx, const std::vector<XzbDecJob> &jobs, uint32
 		// Delta / BCJ behind LZMA2 (common/filter_decoder.c:44-139): undone in reverse chain order over what each Block
 		// produced, before the integrity check looks at the bytes
 		uint32_t depth = 0;
-		for (const HostBlock &hb : *chains) depth = std::max(depth, hb.n_pre);
+		for (const XzbBlockHeader &hb : *chains) depth = std::max(depth, hb.n_pre);
 		for (uint32_t lvl = 0; lvl < depth; ++lvl) {
 			std::vector<XzbFiltJob> fj(B);
 			for (uint32_t b = 0; b < B; ++b) {
-				const HostBlock &hb = (*chains)[b];
+				const XzbBlockHeader &hb = (*chains)[b];
 				fj[b] = XzbFiltJob{ jobs[b].out, jobs[b].out, 0, 0, 0, 0 };
 				if (lvl < hb.n_pre) { const XzbPreFilter f = hb.pre[hb.n_pre - 1 - lvl]; fj[b].size = results[b].out_used; fj[b].id = f.id; fj[b].arg = f.arg; }
 			}
@@ -1324,72 +1317,6 @@ extern "C" int xzb_decode_blocks_device(xzb_ctx *ctx, const void *d_in, const ui
 	return XZB_OK;
 }
 
-static uint32_t rd32(const uint8_t *p) { return p[0] | ((uint32_t)p[1] << 8) | ((uint32_t)p[2] << 16) | ((uint32_t)p[3] << 24); }
-
-// lzma_vli_decode (single call), common/vli_decoder.c:16-86.  Returns 0 ok, 1 need more, 2 bad.
-static int vli_get(const uint8_t *in, uint64_t *pos, uint64_t size, uint64_t *v)
-{
-	*v = 0;
-	for (uint32_t i = 0; i < 9; ++i) {
-		if (*pos >= size) return 1;
-		const uint8_t b = in[(*pos)++];
-		*v |= (uint64_t)(b & 0x7F) << (7 * i);
-		if ((b & 0x80) == 0) return (b == 0x00 && i != 0) ? 2 : 0;
-	}
-	return 2;
-}
-
-
-// Block Header, common/block_header_decoder.c:17-124 (LZMA2-only chains are in scope)
-static int parse_block_header(const xzb_ctx *ctx, const uint8_t *in, uint64_t ip, uint64_t in_size, HostBlock *hb)
-{
-	const uint32_t hsize = ((uint32_t)in[ip] + 1) * 4;
-	if (in_size - ip < hsize) return XZB_BUF_ERROR;
-	const uint8_t *h = in + ip;
-	const uint64_t hin = hsize - 4;
-	if (xzb_crc32_bytes(ctx->h_tab.crc32, h, (uint32_t)hin, 0) != rd32(h + hin)) return XZB_DATA_ERROR;
-	if (h[1] & 0x3C) return XZB_OPTIONS_ERROR;
-	uint64_t hp = 2;
-	hb->comp = UINT64_MAX; hb->uncomp = UINT64_MAX;
-	if (h[1] & 0x40) {
-		if (vli_get(h, &hp, hin, &hb->comp) != 0) return XZB_DATA_ERROR;
-		if (hb->comp == 0 || hb->comp > (UINT64_MAX / 2 - 1024 - 64 - 4)) return XZB_DATA_ERROR;
-	}
-	if (h[1] & 0x80) { if (vli_get(h, &hp, hin, &hb->uncomp) != 0) return XZB_DATA_ERROR; }
-	const uint32_t nfilters = (h[1] & 3) + 1;
-	bool have = false;
-	hb->n_pre = 0;
-	for (uint32_t f = 0; f < nfilters; ++f) {  // lzma_filter_flags_decode, filter_flags_decoder.c:16-45
-		uint64_t id, psize;
-		if (vli_get(h, &hp, hin, &id) != 0 || id >= (1ull << 62)) return XZB_DATA_ERROR;
-		if (vli_get(h, &hp, hin, &psize) != 0 || hin - hp < psize) return XZB_DATA_ERROR;
-		if (f + 1 < nfilters) {
-			// a filter in front of the last one: Delta or BCJ (LZMA2 may only be last, validate_chain, filter_common.c:122-249)
-			if (id > 0xFF || !xzb_filter_known((uint32_t)id)) return XZB_OPTIONS_ERROR;
-			XzbPreFilter &pf = hb->pre[hb->n_pre++];
-			pf.id = (uint32_t)id; pf.arg = 0;
-			if (id == XZB_FILTER_DELTA) {          // lzma_delta_props_decode, delta_decoder.c:66-87
-				if (psize != 1) return XZB_OPTIONS_ERROR;
-				pf.arg = (uint32_t)h[hp] + 1;
-			} else {                               // lzma_simple_props_decode, simple_decoder.c:15-39
-				if (psize == 4) pf.arg = rd32(h + hp);
-				else if (psize != 0) return XZB_OPTIONS_ERROR;
-				if (pf.arg & (xzb_filter_alignment(pf.id) - 1)) return XZB_OPTIONS_ERROR;
-			}
-			hp += psize;
-			continue;
-		}
-		if (id != 0x21) return XZB_OPTIONS_ERROR;
-		if (psize != 1 || (h[hp] & 0xC0) || h[hp] > 40) return XZB_OPTIONS_ERROR;  // lzma_lzma2_props_decode, lzma2_decoder.c:298-331
-		hb->dict_size = h[hp] == 40 ? 0xFFFFFFFFu : (2u | (h[hp] & 1u)) << (h[hp] / 2u + 11);
-		hp += psize; have = true;
-	}
-	while (hp < hin) if (h[hp++] != 0x00) return XZB_OPTIONS_ERROR;
-	if (!have) return XZB_OPTIONS_ERROR;
-	hb->hdr_off = ip; hb->hsize = hsize;
-	return XZB_OK;
-}
-
 // lzma_raw_decoder_memusage() of the reference for an LZMA2 Block (filter_decoder.c:208-214 ->
 // lzma2_decoder.c:291-295 -> lzma_decoder.c:1215-1220 -> lz_decoder.c:329-333, + LZMA_MEMUSAGE_BASE): the
 // dictionary plus 66200 bytes of coder structures on the reference's LP64 build.  Walks the sized
@@ -1402,12 +1329,11 @@ extern "C" int xzb_stream_memusage(xzb_ctx *ctx, const uint8_t *in, uint64_t in_
 	*memusage = 32768;  // LZMA_MEMUSAGE_BASE, common.h:68
 	*exceeds = 0;
 	if (in_size < 12) return XZB_OK;
-	static const uint8_t check_sizes[16] = { 0, 4, 4, 4, 8, 8, 8, 16, 16, 16, 32, 32, 32, 64, 64, 64 };
-	const uint32_t csize = check_sizes[in[7] & 0x0F];
+	const uint32_t csize = xzb_check_field_size(in[7] & 0x0F);
 	uint64_t ip = 12;
 	while (ip < in_size && in[ip] != 0x00) {
-		HostBlock hb;
-		if (parse_block_header(ctx, in, ip, in_size, &hb) != XZB_OK) break;
+		XzbBlockHeader hb;
+		if (xzb_block_header_decode(ctx->h_tab.crc32, in + ip, in_size - ip, &hb) != XZB_OK) break;
 		*memusage = (uint64_t)hb.dict_size + 66200;
 		if (*memusage > limit) { *exceeds = 1; break; }
 		if (hb.comp == UINT64_MAX) break;  // unsized Block: its end is only known by decoding it
@@ -1462,19 +1388,15 @@ extern "C" int xzb_stream_decode_prior(xzb_ctx *ctx, const uint8_t *in, uint64_t
 	ctx->err[0] = 0;
 	*out_size = 0;
 	cudaStream_t st = ctx->stream;
-	static const uint8_t magic[6] = { 0xFD, 0x37, 0x7A, 0x58, 0x5A, 0x00 };
 	// XZB_BUF_ERROR has two causes that the one-shot API tells apart (stream_buffer_decoder.c:56-71):
 	// 1 = the input ended early, 2 = the output buffer is too small.
 	ctx->dec_buf_reason = 1;
 	int buf_reason = 1;
-	// Stream Header: common/stream_flags_decoder.c:26-60
 	if (in_size < 12) return XZB_BUF_ERROR;
-	if (memcmp(in, magic, 6) != 0) return XZB_FORMAT_ERROR;
-	if (xzb_crc32_bytes(ctx->h_tab.crc32, in + 6, 2, 0) != rd32(in + 8)) return XZB_DATA_ERROR;
-	if (in[6] != 0x00 || (in[7] & 0xF0)) return XZB_OPTIONS_ERROR;
-	const uint32_t check = in[7] & 0x0F;
-	static const uint8_t check_sizes[16] = { 0, 4, 4, 4, 8, 8, 8, 16, 16, 16, 32, 32, 32, 64, 64, 64 };
-	const uint32_t csize = check_sizes[check];
+	uint32_t check = 0;
+	const int hr = xzb_stream_header_decode(ctx->h_tab.crc32, in, &check);
+	if (hr != XZB_OK) return hr;
+	const uint32_t csize = xzb_check_field_size(check);
 	// Checks other than CRC32 / CRC64 / SHA-256 are reserved IDs: like the reference
 	// (block_decoder.c:178-190 compares only when lzma_check_is_supported()) they are skipped.
 	const bool verify = !(flags & XZB_DEC_IGNORE_CHECK);  // LZMA_IGNORE_CHECK, stream_decoder.c:188-190
@@ -1494,19 +1416,19 @@ extern "C" int xzb_stream_decode_prior(xzb_ctx *ctx, const uint8_t *in, uint64_t
 	bool at_index = false;
 	while (!at_index) {
 		// gather a batch of blocks whose headers carry both sizes (stream_decoder_mt.c:862-931)
-		std::vector<HostBlock> batch;
-		std::vector<uint64_t> out_offs;
+		std::vector<XzbBlockHeader> batch;
+		std::vector<uint64_t> hdr_offs, out_offs;
 		uint64_t bip = ip, bop = op;
 		int pending = XZB_OK;  // error discovered while scanning ahead: report after the batch
 		for (;;) {
 			if (bip >= in_size) { pending = XZB_BUF_ERROR; break; }
 			if (in[bip] == 0x00) { at_index = true; break; }
-			HostBlock hb;
-			const int r = parse_block_header(ctx, in, bip, in_size, &hb);
+			XzbBlockHeader hb;
+			const int r = xzb_block_header_decode(ctx->h_tab.crc32, in + bip, in_size - bip, &hb);
 			if (r != XZB_OK) { pending = r; break; }
 			const bool sized = hb.comp != UINT64_MAX && hb.uncomp != UINT64_MAX;
 			if (!sized && !batch.empty()) break;  // decode what we have first
-			batch.push_back(hb); out_offs.push_back(bop);
+			batch.push_back(hb); hdr_offs.push_back(bip); out_offs.push_back(bop);
 			if (!sized) break;  // direct mode: one block at a time
 			const uint64_t padded = (hb.comp + 3) & ~3ull;
 			if (in_size - (bip + hb.hsize) < padded + csize || out_cap - bop < hb.uncomp) break;  // let the per-block logic report it
@@ -1517,8 +1439,8 @@ extern "C" int xzb_stream_decode_prior(xzb_ctx *ctx, const uint8_t *in, uint64_t
 		std::vector<XzbDecJob> jobs(batch.size());
 		std::vector<bool> truncated(batch.size()), out_exact(batch.size());
 		for (size_t b = 0; b < batch.size(); ++b) {
-			const HostBlock &hb = batch[b];
-			const uint64_t dpos = hb.hdr_off + hb.hsize;
+			const XzbBlockHeader &hb = batch[b];
+			const uint64_t dpos = hdr_offs[b] + hb.hsize;
 			uint64_t in_avail = in_size - dpos; truncated[b] = true;
 			if (hb.comp != UINT64_MAX && hb.comp <= in_avail) { in_avail = hb.comp; truncated[b] = false; }
 			uint64_t out_limit = out_cap - out_offs[b]; out_exact[b] = false;
@@ -1529,21 +1451,21 @@ extern "C" int xzb_stream_decode_prior(xzb_ctx *ctx, const uint8_t *in, uint64_t
 		}
 		std::vector<XzbDecResult> results; std::vector<uint64_t> crcs; std::vector<uint8_t> shas;
 		bool any_chain = false;
-		for (const HostBlock &hb : batch) any_chain = any_chain || hb.n_pre != 0;
+		for (const XzbBlockHeader &hb : batch) any_chain = any_chain || hb.n_pre != 0;
 		int r = decode_batch(ctx, jobs, verify ? check : 0, results, crcs, &shas, any_chain ? &batch : nullptr);
 		if (r != XZB_OK) return r;
 		// per-block validation in stream order: common/block_decoder.c:64-200.  Like the reference
 		// (lz_decoder.c:128-160 copies what was decoded before it looks at the return code), the bytes a
 		// failing Block produced before the error are still delivered.
 		for (size_t b = 0; b < batch.size() && ret == XZB_OK; ++b) {
-			const HostBlock &hb = batch[b];
+			const XzbBlockHeader &hb = batch[b];
 			const XzbDecResult &res = results[b];
 			const uint64_t op_fail = out_offs[b] + res.out_used;
 			if (res.ret == XZB_NEED_INPUT) ret = truncated[b] ? XZB_BUF_ERROR : XZB_DATA_ERROR;
 			else if (res.ret == XZB_NEED_OUTPUT) { ret = out_exact[b] ? XZB_DATA_ERROR : XZB_BUF_ERROR; buf_reason = 2; }
 			else if (res.ret != XZB_OK) ret = (int)res.ret;
 			else if ((hb.comp != UINT64_MAX && res.in_used != hb.comp) || (hb.uncomp != UINT64_MAX && res.out_used != hb.uncomp)) ret = XZB_DATA_ERROR;
-			uint64_t p = hb.hdr_off + hb.hsize + res.in_used;
+			uint64_t p = hdr_offs[b] + hb.hsize + res.in_used;
 			uint64_t c = res.in_used;
 			while (ret == XZB_OK && (c & 3)) {
 				if (p >= in_size) ret = XZB_BUF_ERROR;
@@ -1552,8 +1474,8 @@ extern "C" int xzb_stream_decode_prior(xzb_ctx *ctx, const uint8_t *in, uint64_t
 			}
 			if (ret == XZB_OK && in_size - p < csize) ret = XZB_BUF_ERROR;
 			if (ret == XZB_OK && verify) {
-				if (check == 1) { if ((uint32_t)crcs[b] != rd32(in + p)) ret = XZB_DATA_ERROR; }
-				else if (check == 4) { if (crcs[b] != ((uint64_t)rd32(in + p) | ((uint64_t)rd32(in + p + 4) << 32))) ret = XZB_DATA_ERROR; }
+				if (check == 1) { if ((uint32_t)crcs[b] != xzb_rd32(in + p)) ret = XZB_DATA_ERROR; }
+				else if (check == 4) { if (crcs[b] != ((uint64_t)xzb_rd32(in + p) | ((uint64_t)xzb_rd32(in + p + 4) << 32))) ret = XZB_DATA_ERROR; }
 				else if (check == 10) { if (memcmp(shas.data() + 32 * b, in + p, 32) != 0) ret = XZB_DATA_ERROR; }
 			}
 			if (ret != XZB_OK) { op = op_fail; break; }
@@ -1568,45 +1490,15 @@ extern "C" int xzb_stream_decode_prior(xzb_ctx *ctx, const uint8_t *in, uint64_t
 	}
 	if (ret == XZB_OK) {
 		// Index + Stream Footer: common/index_hash.c:175-341, stream_decoder.c:266-332
-		const uint64_t istart = ip;
-		++ip;
-		uint64_t count = 0;
-		int v = vli_get(in, &ip, in_size, &count);
-		if (v != 0) ret = v == 1 ? XZB_BUF_ERROR : XZB_DATA_ERROR;
-		else if (count != recs.size()) ret = XZB_DATA_ERROR;
-		for (size_t i = 0; ret == XZB_OK && i < recs.size(); ++i) {
-			uint64_t u = 0, w = 0;
-			v = vli_get(in, &ip, in_size, &u);
-			if (v == 0) v = vli_get(in, &ip, in_size, &w);
-			if (v != 0) { ret = v == 1 ? XZB_BUF_ERROR : XZB_DATA_ERROR; break; }
-			if (u != recs[i].unpadded_size || w != recs[i].uncompressed_size) ret = XZB_DATA_ERROR;
-		}
-		while (ret == XZB_OK && ((ip - istart) & 3)) {
-			if (ip >= in_size) ret = XZB_BUF_ERROR;
-			else if (in[ip++] != 0x00) ret = XZB_DATA_ERROR;
-		}
-		if (ret == XZB_OK) {
-			if (in_size - ip < 4) ret = XZB_BUF_ERROR;
-			else {
-				uint32_t crc = 0xFFFFFFFFu;
-				for (uint64_t i = istart; i < ip; ++i) crc = ctx->h_tab.crc32[(crc ^ in[i]) & 0xFF] ^ (crc >> 8);
-				if (~crc != rd32(in + ip)) ret = XZB_DATA_ERROR;
-				ip += 4;
-			}
-		}
-		if (ret == XZB_OK) {
-			const uint64_t isize = ip - istart;
-			if (in_size - ip < 12) ret = XZB_BUF_ERROR;
-			else {
-				const uint8_t *f = in + ip;
-				if (f[10] != 'Y' || f[11] != 'Z') ret = XZB_DATA_ERROR;
-				else if (xzb_crc32_bytes(ctx->h_tab.crc32, f + 4, 6, 0) != rd32(f)) ret = XZB_DATA_ERROR;
-				else if (f[8] != 0x00 || (f[9] & 0xF0)) ret = XZB_OPTIONS_ERROR;
-				else if (((uint64_t)rd32(f + 4) + 1) * 4 != isize) ret = XZB_DATA_ERROR;
-				else if ((uint32_t)(f[9] & 0x0F) != check) ret = XZB_DATA_ERROR;
-				else ip += 12;
-			}
-		}
+		const XzbIndexWant want{ recs.data(), recs.size() };
+		XzbIndexRead x;
+		ret = xzb_index_read(ctx->h_tab.crc32, in + ip, in_size - ip, &want, &x);
+		ip += x.stop;
+		uint32_t fcheck = 0; uint64_t fisize = 0;
+		if (ret == XZB_OK && in_size - ip < 12) ret = XZB_BUF_ERROR;
+		if (ret == XZB_OK) ret = xzb_stream_footer_decode(ctx->h_tab.crc32, in + ip, &fcheck, &fisize);
+		if (ret == XZB_OK && (fisize != x.end || fcheck != check)) ret = XZB_DATA_ERROR;
+		if (ret == XZB_OK) ip += 12;
 	}
 	*in_used = ip;
 	ctx->dec_buf_reason = buf_reason;

@@ -13,6 +13,7 @@
 
 #include "../../include/xzb200.h"
 #include "../../include/xzb200_lzma.h"
+#include "xzb_params.h"
 
 namespace {
 
@@ -319,35 +320,33 @@ lzma_ret encoder_code(GpuCoder *in, const uint8_t *src, size_t *in_pos, size_t i
 	return in->outq.empty() ? LZMA_STREAM_END : LZMA_OK;
 }
 
+const uint32_t *crc32_table()  // for the container readers of xzb_frame.cuh
+{
+	static const XzbHostTables t = [] { XzbHostTables h; xzb_make_tables(&h); return h; }();
+	return t.crc32;
+}
+
 // Is a whole Stream (header .. footer) buffered?  Walks sized Block Headers only; unsized Blocks
-// (single-threaded encoders) are only known to be complete at LZMA_FINISH.
+// (single-threaded encoders) are only known to be complete at LZMA_FINISH.  Lax on purpose (the decoder validates):
+// a Compressed Size counts as far as it goes unless it has no last byte within nine.
 bool stream_complete(const std::vector<uint8_t> &b, size_t *end)
 {
 	if (b.size() < 12) return false;
+	const uint32_t csize = xzb_check_field_size(b[7] & 0x0F);
 	size_t ip = 12;
 	for (;;) {
 		if (ip >= b.size()) return false;
 		if (b[ip] == 0x00) break;
-		const size_t hs = ((size_t)b[ip] + 1) * 4;
-		if (b.size() - ip < hs) return false;
-		if ((b[ip + 1] & 0x40) == 0) return false;
-		uint64_t comp = 0; size_t p = ip + 2; unsigned i = 0;
-		for (; i < 9 && p < ip + hs; ++i) { const uint8_t c = b[p++]; comp |= (uint64_t)(c & 0x7F) << (7 * i); if (!(c & 0x80)) break; }
-		if (i == 9) return false;
-		static const uint8_t cs[16] = { 0, 4, 4, 4, 8, 8, 8, 16, 16, 16, 32, 32, 32, 64, 64, 64 };
-		const uint64_t total = hs + ((comp + 3) & ~3ull) + cs[b[7] & 0x0F];
+		XzbBlockFraming f;
+		if (!xzb_block_framing(b.data() + ip, b.size() - ip, &f) || !(f.flags & 0x40) || f.comp.st == XZB_VLI_LONG) return false;
+		const uint64_t total = f.hsize + ((f.comp.v + 3) & ~3ull) + csize;
 		if (b.size() - ip < total) return false;
 		ip += (size_t)total;
 	}
-	// Index: 0x00, count, records, padding, crc32; then 12-byte footer whose Backward Size gives the Index size
-	size_t p = ip + 1; uint64_t count = 0; unsigned i = 0;
-	for (; i < 9; ++i) { if (p >= b.size()) return false; const uint8_t c = b[p++]; count |= (uint64_t)(c & 0x7F) << (7 * i); if (!(c & 0x80)) break; }
-	for (uint64_t r = 0; r < count * 2; ++r) {
-		for (i = 0; i < 9; ++i) { if (p >= b.size()) return false; if (!(b[p++] & 0x80)) break; }
-	}
-	p = ip + (((p - ip) + 3) & ~(size_t)3) + 4;
-	if (b.size() < p + 12) return false;
-	*end = p + 12;
+	XzbIndexRead x;
+	xzb_index_read(crc32_table(), b.data() + ip, b.size() - ip, nullptr, &x);
+	if (!x.listed || b.size() - ip < x.end + 12) return false;
+	*end = ip + (size_t)x.end + 12;
 	return true;
 }
 
@@ -357,48 +356,44 @@ const uint64_t MAX_RATIO = 8192;
 
 // First guess of a Stream's uncompressed size from its Block Headers.  Header fields come from untrusted input, so a
 // claimed size counts only as far as the compressed bytes can justify it; unsized Blocks start from a modest guess and
-// the caller grows the buffer when the decoder reports that the output did not fit.
+// the caller grows the buffer when the decoder reports that the output did not fit.  Walks as stream_complete did.
 uint64_t stream_out_bound(const std::vector<uint8_t> &b, size_t off, size_t len, bool complete)
 {
 	if (!complete) return (uint64_t)len * 16 + (1u << 20);
 	uint64_t cap = 0;
 	size_t ip = off + 12;
-	static const uint8_t cs[16] = { 0, 4, 4, 4, 8, 8, 8, 16, 16, 16, 32, 32, 32, 64, 64, 64 };
+	const uint32_t csize = xzb_check_field_size(b[off + 7] & 0x0F);
 	while (b[ip] != 0x00) {
-		const size_t hs = ((size_t)b[ip] + 1) * 4;
-		size_t p = ip + 2; uint64_t comp = 0, unc = 0; unsigned i;
-		for (i = 0; i < 9; ++i) { const uint8_t c = b[p++]; comp |= (uint64_t)(c & 0x7F) << (7 * i); if (!(c & 0x80)) break; }
-		if (b[ip + 1] & 0x80) for (i = 0; i < 9; ++i) { const uint8_t c = b[p++]; unc |= (uint64_t)(c & 0x7F) << (7 * i); if (!(c & 0x80)) break; }
-		else unc = comp * 16 + 65536;
-		if (unc > comp * MAX_RATIO + 65536) unc = comp * MAX_RATIO + 65536;
+		XzbBlockFraming f;
+		xzb_block_framing(b.data() + ip, b.size() - ip, &f);
+		uint64_t unc = (f.flags & 0x80) ? f.uncomp.v : f.comp.v * 16 + 65536;
+		if (unc > f.comp.v * MAX_RATIO + 65536) unc = f.comp.v * MAX_RATIO + 65536;
 		cap += unc;
-		ip += hs + (size_t)((comp + 3) & ~3ull) + cs[b[off + 7] & 0x0F];
+		ip += f.hsize + (size_t)((f.comp.v + 3) & ~3ull) + csize;
 	}
 	return cap;
 }
 
 // Complete sized Blocks at the front of an incomplete Stream (b = Stream Header + Blocks so far): how many,
-// where they end, their uncompressed total, and their Index records as the headers state them.
+// where they end, their uncompressed total, and their Index records as the headers state them.  Lax like
+// stream_complete, except that the Compressed Size must end inside the header, before the Uncompressed Size.
 static size_t complete_blocks(const std::vector<uint8_t> &b, size_t *end, uint64_t *unc_total, std::vector<xzb_index_record> *recs)
 {
-	static const uint8_t cs[16] = { 0, 4, 4, 4, 8, 8, 8, 16, 16, 16, 32, 32, 32, 64, 64, 64 };
 	size_t n = 0, ip = 12;
 	*end = 12; *unc_total = 0;
 	if (b.size() < 12) return 0;
-	const size_t csize = cs[b[7] & 0x0F];
+	const size_t csize = xzb_check_field_size(b[7] & 0x0F);
 	while (ip < b.size() && b[ip] != 0x00) {
-		const size_t hs = ((size_t)b[ip] + 1) * 4;
-		if (b.size() - ip < hs || (b[ip + 1] & 0xC0) != 0xC0) break;  // both sizes must be in the header
-		uint64_t comp = 0, unc = 0; size_t p = ip + 2; unsigned i;
-		for (i = 0; i < 9 && p < ip + hs; ++i) { const uint8_t c = b[p++]; comp |= (uint64_t)(c & 0x7F) << (7 * i); if (!(c & 0x80)) break; }
-		if (i == 9 || p >= ip + hs) break;
-		for (i = 0; i < 9 && p < ip + hs; ++i) { const uint8_t c = b[p++]; unc |= (uint64_t)(c & 0x7F) << (7 * i); if (!(c & 0x80)) break; }
-		if (i == 9 || comp == 0 || comp > (1ull << 40) || unc > comp * MAX_RATIO + 65536) break;  // a size the payload cannot justify is left to the final pass
-		const uint64_t total = hs + ((comp + 3) & ~3ull) + csize;
+		XzbBlockFraming f;
+		if (!xzb_block_framing(b.data() + ip, b.size() - ip, &f) || (f.flags & 0xC0) != 0xC0) break;  // both sizes must be in the header
+		const uint64_t comp = f.comp.v, unc = f.uncomp.v;
+		if (f.comp.st == XZB_VLI_LONG || f.comp.end >= f.hsize || f.uncomp.st == XZB_VLI_LONG) break;
+		if (comp == 0 || comp > (1ull << 40) || unc > comp * MAX_RATIO + 65536) break;  // a size the payload cannot justify is left to the final pass
+		const uint64_t total = f.hsize + ((comp + 3) & ~3ull) + csize;
 		if (b.size() - ip < total) break;
 		ip += (size_t)total;
 		*unc_total += unc;
-		recs->push_back(xzb_index_record{ hs + comp + csize, unc });
+		recs->push_back(xzb_index_record{ f.hsize + comp + csize, unc });
 		++n; *end = ip;
 	}
 	return n;
@@ -412,10 +407,8 @@ static uint32_t dec_flags(uint32_t lzma_flags)
 // Check ID of a valid Stream Header at p (12 bytes), or -1.
 static int header_check_id(const uint8_t *p)
 {
-	if (p[7] & 0xF0) return -1;
-	uint8_t want[12];
-	xzb_stream_header_encode(want, p[7] & 0x0F);
-	return memcmp(p, want, 12) == 0 ? (int)(p[7] & 0x0F) : -1;
+	uint32_t check = 0;
+	return xzb_stream_header_decode(crc32_table(), p, &check) == XZB_OK ? (int)check : -1;
 }
 
 // Do the buffered bytes end in a valid Stream Footer (stream_flags_decoder.c:51-83)?  Used under LZMA_RUN to notice
@@ -423,12 +416,8 @@ static int header_check_id(const uint8_t *p)
 static bool footer_at_end(const std::vector<uint8_t> &b)
 {
 	if (b.size() < 32 || (b.size() & 3) != 0) return false;
-	const uint8_t *f = b.data() + b.size() - 12;
-	if (f[10] != 'Y' || f[11] != 'Z' || f[8] != 0 || (f[9] & 0xF0) != 0) return false;
-	const uint64_t backward = ((uint64_t)f[4] | ((uint64_t)f[5] << 8) | ((uint64_t)f[6] << 16) | ((uint64_t)f[7] << 24));
-	uint8_t want[12];
-	xzb_stream_footer_encode(want, f[9] & 0x0F, (backward + 1) * 4);
-	return memcmp(f, want, 12) == 0;
+	uint32_t check = 0; uint64_t index_size = 0;
+	return xzb_stream_footer_decode(crc32_table(), b.data() + b.size() - 12, &check, &index_size) == XZB_OK;
 }
 
 // stream_decode, common/stream_decoder.c:101-378, as a resumable loop over the buffered input: a
@@ -584,8 +573,7 @@ lzma_bool lzma_check_is_supported(lzma_check check)
 }
 uint32_t lzma_check_size(lzma_check check)
 {
-	static const uint8_t cs[16] = { 0, 4, 4, 4, 8, 8, 8, 16, 16, 16, 32, 32, 32, 64, 64, 64 };
-	return (unsigned)check > 15 ? UINT32_MAX : cs[(unsigned)check];
+	return xzb_check_field_size((uint32_t)check);
 }
 size_t lzma_block_buffer_bound(size_t uncompressed_size) { return (size_t)xzb_block_bound(uncompressed_size); }
 
@@ -670,14 +658,11 @@ lzma_ret lzma_block_buffer_encode(lzma_block *block, const lzma_allocator *alloc
 	if (!to_xzb_options((const lzma_options_lzma *)f[0].options, &x) || !valid_lzma2_options(x)) return LZMA_OPTIONS_ERROR;
 	if (in_size > ((size_t)1 << 30)) return LZMA_OPTIONS_ERROR;  // GPU path limit (DESIGN.md)
 	std::vector<uint8_t> tmp;
-	const uint8_t *blk = nullptr;
-	size_t total = 0;
+	size_t at = 0;  // the Block in tmp
 	if (in_size == 0) {
 		// nothing to search or code: header + the LZMA2 end marker alone (lzma2_encoder.c:141-150)
 		tmp.resize(64 + check_size);
 		tmp.resize(xzb_empty_block_encode(tmp.data(), &x, (uint32_t)block->check));
-		const uint8_t *h = tmp.data();
-		blk = h; total = tmp.size();
 	} else {
 		std::lock_guard<std::mutex> lock(g_oneshot_mu);
 		xzb_ctx *ctx = nullptr;
@@ -688,19 +673,17 @@ lzma_ret lzma_block_buffer_encode(lzma_block *block, const lzma_allocator *alloc
 		uint64_t produced = 0;
 		const int r = xzb_stream_buffer_encode(ctx, in, in_size, &x, (uint32_t)block->check, tmp.data(), bound, &produced);
 		if (r != 0) return (lzma_ret)r;
-		blk = tmp.data() + 12;
-		const size_t hs = ((size_t)blk[0] + 1) * 4;
-		uint64_t comp = 0; unsigned i = 0; size_t p = 2;
-		for (; i < 9; ++i) { const uint8_t c = blk[p++]; comp |= (uint64_t)(c & 0x7F) << (7 * i); if (!(c & 0x80)) break; }
-		total = hs + (size_t)((comp + 3) & ~3ull) + check_size;
+		at = 12;
 	}
+	const uint8_t *blk = tmp.data() + at;
+	XzbBlockFraming hdr;  // a header this library wrote: both sizes are in it
+	xzb_block_framing(blk, tmp.size() - at, &hdr);
+	const size_t total = hdr.hsize + (size_t)((hdr.comp.v + 3) & ~3ull) + check_size;
 	if (total > room) return LZMA_BUF_ERROR;
-	const size_t hs = ((size_t)blk[0] + 1) * 4;
-	uint64_t comp = 0; { unsigned i = 0; size_t p = 2; for (; i < 9; ++i) { const uint8_t c = blk[p++]; comp |= (uint64_t)(c & 0x7F) << (7 * i); if (!(c & 0x80)) break; } }
 	memcpy(out + *out_pos, blk, total);
 	*out_pos += total;
-	block->header_size = (uint32_t)hs;
-	block->compressed_size = comp;
+	block->header_size = hdr.hsize;
+	block->compressed_size = hdr.comp.v;
 	block->uncompressed_size = in_size;
 	memcpy(block->raw_check, blk + total - check_size, check_size);
 	return LZMA_OK;
@@ -737,15 +720,9 @@ lzma_ret lzma_stream_buffer_decode(uint64_t *memlimit, uint32_t flags, const lzm
 	for (;;) {
 		// LZMA_TELL_NO_CHECK / LZMA_TELL_UNSUPPORTED_CHECK after a valid Stream Header
 		// (stream_decoder.c:139-151): the code is not LZMA_STREAM_END, so the one-shot call fails with it
-		if (in_size - ip >= 12 && (in[ip + 7] & 0xF0) == 0) {
-			const uint32_t chk = in[ip + 7] & 0x0F;
-			uint8_t want[12];
-			xzb_stream_header_encode(want, chk);
-			if (memcmp(in + ip, want, 12) == 0) {
-				if ((flags & LZMA_TELL_NO_CHECK) && chk == 0) return LZMA_NO_CHECK;
-				if ((flags & LZMA_TELL_UNSUPPORTED_CHECK) && !lzma_check_is_supported((lzma_check)chk)) return LZMA_UNSUPPORTED_CHECK;
-			}
-		}
+		const int chk = in_size - ip >= 12 ? header_check_id(in + ip) : -1;
+		if ((flags & LZMA_TELL_NO_CHECK) && chk == 0) return LZMA_NO_CHECK;
+		if ((flags & LZMA_TELL_UNSUPPORTED_CHECK) && chk >= 0 && !lzma_check_is_supported((lzma_check)chk)) return LZMA_UNSUPPORTED_CHECK;
 		uint64_t produced = 0, used = 0;
 		int r = xzb_stream_buffer_decode(ctx, in + ip, in_size - ip, out ? out + op : dummy_out, out_size - op, &produced, &used, dec_flags(flags));
 		if (r == 7 && !first) r = 9;  // LZMA_FORMAT_ERROR in a later Stream is LZMA_DATA_ERROR (stream_decoder.c:121-123)
