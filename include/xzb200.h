@@ -132,6 +132,24 @@ int xzb_stream_buffer_encode(xzb_ctx *ctx, const uint8_t *in, uint64_t in_size,
 		const xzb_lzma_options *opt, uint32_t check,
 		uint8_t *out, uint64_t out_cap, uint64_t *out_size);
 
+/*
+ * ENCODE, batch of n independent one-shot Streams (liblzma has no such call: this is n lzma_stream_buffer_encode()
+ * calls at once).  Item i is in[in_off[i] .. in_off[i] + in_size[i]); its Stream goes to out + out_off[i] (room:
+ * out_cap[i]); out_size[i] and ret[i] are what xzb_stream_buffer_encode() gives for that item alone with out_cap[i]
+ * -- same bytes, same codes (XZB_BUF_ERROR when it does not fit, XZB_OPTIONS_ERROR above 1 GiB); an item that fails
+ * gets out_size[i] = 0 and nothing is written to its slot.  Options, check and the context's Delta/BCJ chain
+ * (xzb_ctx_set_filters) apply to every item.  n = 0 and zero-length items are valid (a zero-length item gives the
+ * 32-byte Stream with no Block).  The Blocks of all items are coded in waves of similar sizes, side by side on the GPU.
+ * The return value is for errors of the whole call (options, check, device).
+ */
+int xzb_stream_buffer_encode_batch(xzb_ctx *ctx, uint32_t n, const uint8_t *in, const uint64_t *in_off,
+		const uint64_t *in_size, const xzb_lzma_options *opt, uint32_t check, uint8_t *out,
+		const uint64_t *out_off, const uint64_t *out_cap, uint64_t *out_size, uint32_t *ret);
+/* The same with `in` and `out` in device memory (the offset / size / result arrays stay on the host). */
+int xzb_stream_buffer_encode_batch_device(xzb_ctx *ctx, uint32_t n, const uint8_t *in, const uint64_t *in_off,
+		const uint64_t *in_size, const xzb_lzma_options *opt, uint32_t check, uint8_t *out,
+		const uint64_t *out_off, const uint64_t *out_cap, uint64_t *out_size, uint32_t *ret);
+
 /* Stream framing around device-encoded Blocks (stream_flags_encoder.c:29-85,
  * index_encoder.c:43-165).  xzb_index_encode(out == NULL) returns the size only. */
 uint32_t xzb_stream_header_encode(uint8_t out[12], uint32_t check);
@@ -178,6 +196,13 @@ int xzb_stream_memusage(xzb_ctx *ctx, const uint8_t *in, uint64_t in_size, uint6
  * buffer that is too small is XZB_BUF_ERROR. */
 int xzb_stream_buffer_decode(xzb_ctx *ctx, const uint8_t *in, uint64_t in_size,
 		uint8_t *out, uint64_t out_cap, uint64_t *out_size, uint64_t *in_used, uint32_t flags);
+/* n independent Streams, host buffers: Stream i is in[in_off[i] .. in_off[i] + in_size[i]), its output goes to
+ * out + out_off[i] (room: out_cap[i]).  Per item, (ret, out_size, in_used, bytes written) == xzb_stream_buffer_decode()
+ * of that item alone with out_cap[i] and `flags`, including bytes delivered before an error.  The Blocks of all
+ * Streams are decoded side by side.  The return value is for errors of the whole call (device). */
+int xzb_stream_buffer_decode_batch(xzb_ctx *ctx, uint32_t n, const uint8_t *in, const uint64_t *in_off,
+		const uint64_t *in_size, uint8_t *out, const uint64_t *out_off, const uint64_t *out_cap,
+		uint64_t *out_size, uint64_t *in_used, uint32_t *ret, uint32_t flags);
 
 /*
  * DECODE, device-resident Blocks: comp_off[i]/comp_size[i] locate Block i's LZMA2 payload

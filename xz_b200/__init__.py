@@ -77,6 +77,12 @@ def lib():
         L.xzb_stream_buffer_decode.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64),
                                                C.POINTER(C.c_uint64), C.c_uint32]
         L.xzb_stream_decode_flags.argtypes = L.xzb_stream_buffer_decode.argtypes
+        P64, P32 = C.POINTER(C.c_uint64), C.POINTER(C.c_uint32)
+        L.xzb_stream_buffer_encode_batch.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, P64, P64, C.POINTER(LzmaOptions), C.c_uint32,
+                                                     C.c_void_p, P64, P64, P64, P32]
+        L.xzb_stream_buffer_encode_batch_device.argtypes = L.xzb_stream_buffer_encode_batch.argtypes
+        L.xzb_stream_buffer_decode_batch.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, P64, P64, C.c_void_p, P64, P64, P64, P64, P32,
+                                                     C.c_uint32]
         L.xzb_stream_decode.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64)]
         L.xzb_decode_blocks_device.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64), C.POINTER(C.c_uint64),
                                                C.POINTER(C.c_uint64), C.POINTER(C.c_uint32), C.c_uint32, C.c_uint32, C.c_void_p,
@@ -194,6 +200,64 @@ class Context:
         sz = C.c_uint64(); used = C.c_uint64()
         r = lib().xzb_stream_buffer_decode(self._h, sp, len(data), out, cap, C.byref(sz), C.byref(used), flags)
         return r, bytes(out[: sz.value]), used.value
+
+    # ---- batches of independent one-shot Streams (xzb_stream_buffer_*_batch) ----
+    def stream_buffer_encode_batch(self, items, preset=6, check=LZMA_CHECK_CRC64, opts=None, caps=None):
+        """One lzma_stream_buffer_encode per item, all in one call: [(ret, Stream bytes)] in item order.
+        caps[i] (default xzb_stream_buffer_bound of the item's size) is item i's output room."""
+        o = opts if opts is not None else lzma_lzma_preset(preset)
+        n = len(items)
+        views = [bytes(x) for x in items]
+        sizes = [len(v) for v in views]
+        caps = [lib().xzb_stream_buffer_bound(s) for s in sizes] if caps is None else list(caps)
+        src = bytearray(b"".join(views)) or bytearray(1)
+        A = C.c_uint64 * max(n, 1)
+        in_off, out_off = A(), A()
+        for i in range(1, n):
+            in_off[i] = in_off[i - 1] + sizes[i - 1]
+            out_off[i] = out_off[i - 1] + caps[i - 1]
+        out = (C.c_uint8 * max(sum(caps), 1))()
+        size, rets = A(), (C.c_uint32 * max(n, 1))()
+        sp, _k = _ptr(src)
+        r = lib().xzb_stream_buffer_encode_batch(self._h, n, sp, in_off, A(*sizes), C.byref(o), check, out, out_off, A(*caps), size, rets)
+        if r != LZMA_OK:
+            raise XzError(r, self._err())
+        raw = C.string_at(out, len(out))
+        return [(rets[i], raw[out_off[i]: out_off[i] + size[i]]) for i in range(n)]
+
+    def stream_buffer_encode_batch_device(self, d_in, in_off, in_size, opts, check, d_out, out_off, out_cap):
+        """The batch on device memory: d_in / d_out are addresses (or CUDA tensors; synchronise their stream first),
+        the offset and size lists stay on the host.  Returns [(ret, Stream size)]; the Streams are at d_out + out_off[i]."""
+        n = len(in_off)
+        A = C.c_uint64 * max(n, 1)
+        size, rets = A(), (C.c_uint32 * max(n, 1))()
+        ip, _k1 = _ptr(d_in)
+        op, _k2 = _ptr(d_out)
+        r = lib().xzb_stream_buffer_encode_batch_device(self._h, n, ip, A(*in_off), A(*in_size), C.byref(opts), check, op, A(*out_off),
+                                                        A(*out_cap), size, rets)
+        if r != LZMA_OK:
+            raise XzError(r, self._err())
+        return [(rets[i], size[i]) for i in range(n)]
+
+    def stream_buffer_decode_batch(self, streams, caps, flags=0):
+        """One lzma_stream_buffer_decode per Stream, all in one call: [(ret, bytes, input bytes used)] in Stream order."""
+        n = len(streams)
+        views = [bytes(x) for x in streams]
+        src = bytearray(b"".join(views)) or bytearray(1)
+        A = C.c_uint64 * max(n, 1)
+        in_off, out_off = A(), A()
+        for i in range(1, n):
+            in_off[i] = in_off[i - 1] + len(views[i - 1])
+            out_off[i] = out_off[i - 1] + caps[i - 1]
+        out = (C.c_uint8 * max(sum(caps), 1))()
+        size, used, rets = A(), A(), (C.c_uint32 * max(n, 1))()
+        sp, _k = _ptr(src)
+        r = lib().xzb_stream_buffer_decode_batch(self._h, n, sp, in_off, A(*[len(v) for v in views]), out, out_off, A(*caps), size, used,
+                                                 rets, flags)
+        if r != LZMA_OK:
+            raise XzError(r, self._err())
+        raw = C.string_at(out, len(out))
+        return [(rets[i], raw[out_off[i]: out_off[i] + size[i]], used[i]) for i in range(n)]
 
     # ---- lzma_stream_decoder + lzma_code(FINISH) on host buffers ----
     def stream_decode_into(self, src, n, dst, cap):

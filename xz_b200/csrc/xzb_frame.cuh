@@ -173,6 +173,42 @@ XZB_HD void xzb_block_finish_raw(const uint32_t *crc32_table, const uint8_t *in,
 	}
 }
 
+// ---- placing finished Blocks (xzb_k_pack_streams) ----
+// Size of the one-Block Stream around a Block of block_size bytes (block_size == 0: the Stream with no Block).
+XZB_HD uint64_t xzb_oneshot_stream_size(uint32_t block_size, uint64_t unpadded, uint64_t uncomp)
+{
+	return 12 + (uint64_t)block_size + xzbi_index_encode(0, &unpadded, &uncomp, block_size ? 1 : 0, 0) + 12;
+}
+
+struct alignas(16) XzbV16 { uint32_t w[4]; };
+
+// Copies the finished Block at `block` (16-byte aligned, a multiple of four bytes long) to dst; with `frame` it becomes
+// a whole one-shot Stream: Stream Header, the Block, its one-record Index, Stream Footer (stream_buffer_encoder.c:
+// 43-140).  block_size == 0 with `frame` is the Stream with no Block.  Work-shared by workers tid in [0, nthreads): the
+// Block moves in 16-byte loads; the stores are 16 bytes wide where dst allows, else 4 or 1.  Returns the bytes written.
+XZB_HD uint64_t xzb_pack_stream(const uint32_t *crc32_table, uint8_t *dst, const uint8_t *block, uint32_t block_size,
+		uint64_t unpadded, uint64_t uncomp, uint32_t check, bool frame, uint32_t tid, uint32_t nthreads)
+{
+	uint8_t *d = dst + (frame ? 12 : 0);
+	const uint32_t nv = block_size / 16;
+	const XzbV16 *src = (const XzbV16 *)block;
+	const uintptr_t da = (uintptr_t)d;
+	for (uint32_t i = tid; i < nv; i += nthreads) {
+		const XzbV16 v = src[i];
+		if ((da & 15) == 0) ((XzbV16 *)d)[i] = v;
+		else if ((da & 3) == 0) for (int k = 0; k < 4; ++k) ((uint32_t *)d)[4 * i + k] = v.w[k];
+		else for (int k = 0; k < 16; ++k) d[16 * i + k] = (uint8_t)(v.w[k >> 2] >> (8 * (k & 3)));
+	}
+	for (uint32_t i = 16 * nv + tid; i < block_size; i += nthreads) d[i] = block[i];
+	if (!frame) return block_size;
+	if (tid == 0) {
+		xzb_stream_header(crc32_table, dst, check);
+		const uint64_t isz = xzbi_index_encode(crc32_table, &unpadded, &uncomp, block_size ? 1 : 0, d + block_size);
+		xzb_stream_footer(crc32_table, d + block_size + isz, check, isz);
+	}
+	return xzb_oneshot_stream_size(block_size, unpadded, uncomp);
+}
+
 // ---- read side (host only), over untrusted input: every reader stays inside the `size` / `avail` bytes it is given ----
 static inline uint32_t xzb_check_field_size(uint32_t check)  // any of the 16 Check IDs, supported or not (check.c:62-86)
 {

@@ -8,6 +8,7 @@
 //   xzb_k_crc                               : CRC64/CRC32 of every block (slice + GF(2) fold)
 //   xzb_k_parse_dp | xzb_k_parse_fast  1 CUDA block / .xz block : parser + range coder + LZMA2 chunker
 //   xzb_k_finalize    1 CUDA block / .xz block : header, padding, check | raw fallback
+//   xzb_k_pack_streams  1 CUDA block / .xz block : the finished Block to its place (+ Stream framing for one-shot items)
 // Decode: xzb_k_decode (1 CUDA block / .xz block) + xzb_k_crc over the output.
 // There is deliberately no CPU path in this file.
 #include <cuda_runtime.h>
@@ -36,24 +37,25 @@
 // Kernels
 // ------------------------------------------------------------------------------------
 
-// grid (ceil(bs/256), B): one thread per block position.  Keys are (block << hbits) | hash;
-// positions that are never inserted (short tail, lz_encoder_mf.c:190-201) get the
-// out-of-range block index B so that they sort behind every real key.
+// Wave layout (xzb_params.h): Block b's positions are [off[b], off[b] + n_b) of every per-position array, off[b] a
+// multiple of 256; tile_block[t] is the Block that positions [256 t, 256 t + 256) belong to.
+// One thread per position of the wave, 256-position tiles.  Keys are (block << hbits) | hash; positions that are never
+// inserted (short tail, lz_encoder_mf.c:190-201, and the padding behind a Block) get the out-of-range block index B so
+// that they sort behind every real key.
 __global__ void __launch_bounds__(256)
-xzb_k_hash_keys(const uint8_t *__restrict__ in, uint32_t bs, uint32_t B, const uint32_t *__restrict__ sizes,
+xzb_k_hash_keys(const XzbMfBlock *__restrict__ blocks, const uint32_t *__restrict__ tile_block, const uint32_t *__restrict__ off, uint32_t B,
 		XzbParams P, const uint32_t *__restrict__ crc, uint32_t hbm,
 		uint32_t *__restrict__ keys_m, uint32_t *__restrict__ keys_2, uint32_t *__restrict__ keys_3,
 		uint32_t *__restrict__ vals, uint32_t *__restrict__ mh)
 {
-	const uint32_t blk = blockIdx.y;
-	const uint32_t p = blockIdx.x * blockDim.x + threadIdx.x;
-	if (p >= bs) return;
-	const size_t g = (size_t)blk * bs + p;
-	const uint32_t n = sizes[blk];
+	const uint32_t blk = tile_block[blockIdx.x];
+	const size_t g = (size_t)blockIdx.x * 256 + threadIdx.x;
+	const uint32_t p = (uint32_t)(g - off[blk]);
+	const uint32_t n = blocks[blk].n;
 	uint32_t km = B << hbm, k2 = B << 10, k3 = B << 16;
 	if (p < n && n - p >= P.hash_bytes) {
 		uint32_t h2 = 0, h3 = 0;
-		const uint32_t hm = xzb_hash(in + g, P, crc, &h2, &h3);
+		const uint32_t hm = xzb_hash(blocks[blk].buf + p, P, crc, &h2, &h3);
 		km = (blk << hbm) | hm; k2 = (blk << 10) | h2; k3 = (blk << 16) | h3;
 	} else if (p < n) {
 		mh[g] = 0;
@@ -67,7 +69,7 @@ xzb_k_hash_keys(const uint8_t *__restrict__ in, uint32_t bs, uint32_t B, const u
 // After a stable sort by key: previous element with the same key is the hash head the
 // reference would have read (lz_encoder_mf.c:372-379).
 __global__ void __launch_bounds__(256)
-xzb_k_prev(const uint32_t *__restrict__ keys, const uint32_t *__restrict__ vals, size_t N, uint32_t hb, uint32_t B, uint32_t bs,
+xzb_k_prev(const uint32_t *__restrict__ keys, const uint32_t *__restrict__ vals, size_t N, uint32_t hb, uint32_t B, const uint32_t *__restrict__ off,
 		uint32_t *__restrict__ prev)
 {
 	const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -78,7 +80,7 @@ xzb_k_prev(const uint32_t *__restrict__ keys, const uint32_t *__restrict__ vals,
 	const uint32_t p = vals[i];
 	uint32_t q = XZB_NONE;
 	if (i > 0 && keys[i - 1] == k) q = vals[i - 1];
-	prev[(size_t)blk * bs + p] = q;
+	prev[(size_t)off[blk] + p] = q;
 }
 
 // Binary-tree work units.  A "run" is the positions of one hash bucket (same block, same hash)
@@ -139,12 +141,14 @@ __global__ void xzb_k_publish(uint32_t *flag, uint32_t value)
 	*(volatile uint32_t *)flag = value;
 }
 
-// Hash chain: grid (ceil(bs/128), B), one thread per position.
+// Hash chain: one thread per position of the wave, 128-position tiles (half a tile of tile_block).
 __global__ void __launch_bounds__(128)
-xzb_k_hc(const XzbMfBlock *__restrict__ blocks, XzbParams P)
+xzb_k_hc(const XzbMfBlock *__restrict__ blocks, const uint32_t *__restrict__ tile_block, const uint32_t *__restrict__ off, XzbParams P)
 {
-	const XzbMfBlock B = blocks[blockIdx.y];
-	const uint32_t p = blockIdx.x * blockDim.x + threadIdx.x;
+	const size_t g = (size_t)blockIdx.x * 128 + threadIdx.x;
+	const uint32_t blk = tile_block[blockIdx.x >> 1];
+	const XzbMfBlock B = blocks[blk];
+	const uint32_t p = (uint32_t)(g - off[blk]);
 	if (p >= B.n) return;
 	xzb_hc_position(B, P, p);
 }
@@ -438,6 +442,22 @@ xzb_k_finalize(const XzbEncJob *__restrict__ jobs, const uint32_t *__restrict__ 
 		xzb_block_finish_raw(crc32_table, job.in, job.in_size, job.out, check, check_bytes + (size_t)b * 32, res, threadIdx.x, blockDim.x);
 }
 
+// Places finished Blocks: one CTA per job copies its Block out of scratch to `dst`; with `frame` the job becomes a whole
+// one-shot Stream (xzb_pack_stream).  src == nullptr with frame: the Stream with no Block.
+struct XzbPackJob {
+	const uint8_t *src;
+	uint8_t *dst;
+	uint64_t unpadded, uncomp;
+	uint32_t size, frame;
+};
+
+__global__ void __launch_bounds__(256)
+xzb_k_pack_streams(const XzbPackJob *__restrict__ jobs, const uint32_t *__restrict__ crc32_table, uint32_t check)
+{
+	const XzbPackJob j = jobs[blockIdx.x];
+	xzb_pack_stream(crc32_table, j.dst, j.src, j.size, j.unpadded, j.uncomp, check, j.frame != 0, threadIdx.x, blockDim.x);
+}
+
 // ---- Delta / BCJ filters over whole Blocks (xzb_filters.cuh) ----
 // One CUDA block per .xz Block and chain stage.  `src != dst` only for the Delta encoder (out of place, so every
 // byte reads its unfiltered predecessor); everything else works in place on `dst`.
@@ -536,6 +556,7 @@ struct xzb_ctx {
 	DevBuf keys_a, keys_b, vals_a, vals_b, keys_2, keys_3, prev2, prev3, prevm, son, mh, mp, ovf, cub_tmp;
 	DevBuf run_start, run_len, run_start_s, run_len_s, small, encs, scratch, in_stage, decs, dec_in, dec_out;
 	DevBuf filt_a, filt_b, filt_jobs;   // Delta / BCJ: filtered copies of a wave's input, per-Block stage jobs
+	DevBuf out_stage, pack_jobs;        // finished Blocks / Streams on their way to host memory, xzb_k_pack_streams jobs
 	std::vector<XzbPreFilter> pre;      // the encoder's filters in front of LZMA2 (xzb_ctx_set_filters)
 	int sm_count = 132;
 	cudaStream_t stream_mf = nullptr;   // match-finder segments run here while the parser consumes them
@@ -677,6 +698,7 @@ extern "C" void xzb_ctx_destroy(xzb_ctx *ctx)
 	free_buf(ctx->seg_meta);
 	free_buf(ctx->trace);
 	free_buf(ctx->filt_a); free_buf(ctx->filt_b); free_buf(ctx->filt_jobs);
+	free_buf(ctx->out_stage); free_buf(ctx->pack_jobs);
 	cudaStreamDestroy(ctx->stream);
 	delete ctx;
 }
@@ -743,32 +765,51 @@ extern "C" uint64_t xzb_index_encode(const xzb_index_record *records, uint64_t c
 // ------------------------------------------------------------------------------------
 static uint32_t bit_length(uint32_t v) { uint32_t n = 0; while (v) { ++n; v >>= 1; } return n; }
 
-static uint32_t scratch_cap_for(uint64_t bs) { return (uint32_t)(bs + bs / 4096 + 70000 + 1024) & ~15u; }
-
 // bytes of workspace per block of size bs (upper bound), used to size waves
 static uint64_t wave_bytes_per_block(uint64_t bs, const XzbParams &P)
 {
-	return bs * (uint64_t)(16 + 8 + 12 + 8 + 4 + 8 * P.mstride + 8) + scratch_cap_for(bs) + 4096;
+	return bs * (uint64_t)(16 + 8 + 12 + 8 + 4 + 8 * P.mstride + 8) + xzb_scratch_cap(bs) + 4096;
 }
 
 static float ev_ms(cudaEvent_t a, cudaEvent_t b) { float ms = 0; cudaEventElapsedTime(&ms, a, b); return ms; }
 
-static int encode_wave(xzb_ctx *ctx, const uint8_t *d_in, uint64_t in_bytes, bool has_slack, uint32_t B, uint32_t bs, const XzbParams &P,
-		uint32_t check, uint64_t block_size_opt, bool oneshot, std::vector<XzbBlockResult> &results)
+// One Block of a wave: its input is d_in[in_off .. in_off + n), `room` bytes of it readable; its framing and scratch.
+struct XzbWaveBlock {
+	uint64_t in_off;
+	uint32_t n, room;
+	uint32_t header_size, oneshot;  // see XzbEncJob
+	uint64_t fit_limit;
+	uint32_t scap;                  // scratch capacity
+};
+
+// Encodes the Blocks `wb` side by side.  results[b] is Block b's outcome; its finished bytes are at
+// ctx->scratch + scratch_off[b].  d_in[0 .. in_bytes) covers every Block's input (the filters copy that span).
+static int encode_wave(xzb_ctx *ctx, const uint8_t *d_in, uint64_t in_bytes, const std::vector<XzbWaveBlock> &wb, const XzbParams &P,
+		uint32_t check, std::vector<XzbBlockResult> &results, std::vector<size_t> &scratch_off)
 {
 	cudaStream_t st = ctx->stream;
-	const size_t N = (size_t)B * bs;
+	const uint32_t B = (uint32_t)wb.size();
+	std::vector<uint32_t> h_n(B), h_off(B);
+	uint32_t bs = 0;  // the largest Block
+	size_t scratch_bytes = 0;
+	scratch_off.resize(B);
+	for (uint32_t b = 0; b < B; ++b) {
+		h_n[b] = wb[b].n; bs = std::max(bs, wb[b].n);
+		scratch_off[b] = scratch_bytes; scratch_bytes += wb[b].scap;
+	}
+	const uint64_t N64 = xzb_wave_offsets(h_n.data(), B, h_off.data());
+	const size_t N = (size_t)N64;
+	const uint32_t ntiles = (uint32_t)(N / XZB_WAVE_ALIGN);
 	const uint32_t hbm = bit_length(P.hash_mask);
 	const uint32_t kbits_m = bit_length(B << hbm), kbits_2 = bit_length(B << 10), kbits_3 = bit_length(B << 16);
-	if (N >= 0xFFFFFFF0ull || kbits_m > 32) return set_err(ctx, XZB_PROG_ERROR, "wave too large");
-	const uint32_t scap = scratch_cap_for(block_size_opt);
+	if (N64 >= 0xFFFFFFF0ull || (uint64_t)B << hbm >= (1ull << 32) || kbits_m > 32) return set_err(ctx, XZB_PROG_ERROR, "wave too large");
 
 	EN(ctx->keys_a, 4 * N); EN(ctx->keys_b, 4 * N); EN(ctx->vals_a, 4 * N); EN(ctx->vals_b, 4 * N);
 	if (P.hash_bytes >= 3) { EN(ctx->keys_2, 4 * N); EN(ctx->prev2, 4 * N); }
 	if (P.hash_bytes >= 4) { EN(ctx->keys_3, 4 * N); EN(ctx->prev3, 4 * N); }
 	if (P.is_bt) EN(ctx->son, 8 * N + 64); else EN(ctx->prevm, 4 * N);
 	EN(ctx->mh, 4 * N); EN(ctx->mp, 8 * (size_t)P.mstride * N); EN(ctx->ovf, 8 * N + 4096);
-	EN(ctx->scratch, (size_t)scap * B);
+	EN(ctx->scratch, scratch_bytes);
 	size_t tmp_sort = 0, tmp_sel = 0, tmp_sort2 = 0;
 	cub::DeviceRadixSort::SortPairs(nullptr, tmp_sort, (uint32_t *)nullptr, (uint32_t *)nullptr, (uint32_t *)nullptr, (uint32_t *)nullptr, (int64_t)N, 0, 32, st);
 	if (P.is_bt) {
@@ -796,10 +837,8 @@ static int encode_wave(xzb_ctx *ctx, const uint8_t *d_in, uint64_t in_bytes, boo
 			if (f.id == XZB_FILTER_DELTA) { dst = bufs[which]; which ^= 1; }   // out of place
 			else if (!owned) { dst = bufs[which]; which ^= 1; CK(cudaMemcpyAsync(dst, d_work, in_bytes, cudaMemcpyDeviceToDevice, st)); src = dst; }
 			else { dst = const_cast<uint8_t *>(d_work); }
-			for (uint32_t b = 0; b < B; ++b) {
-				const uint64_t off = (uint64_t)b * bs;
-				fj[s * B + b] = XzbFiltJob{ src + off, dst + off, (uint32_t)std::min<uint64_t>(bs, in_bytes - off), f.id, f.arg, 0 };
-			}
+			for (uint32_t b = 0; b < B; ++b)
+				fj[s * B + b] = XzbFiltJob{ src + wb[b].in_off, dst + wb[b].in_off, wb[b].n, f.id, f.arg, 0 };
 			d_work = dst; owned = true;
 		}
 		CK(cudaMemcpyAsync(ctx->filt_jobs.p, fj.data(), sizeof(XzbFiltJob) * fj.size(), cudaMemcpyHostToDevice, st));
@@ -811,8 +850,8 @@ static int encode_wave(xzb_ctx *ctx, const uint8_t *d_in, uint64_t in_bytes, boo
 	}
 
 	// small per-wave arrays in one allocation
-	const size_t off_sizes = 0;
-	const size_t off_blocks = off_sizes + ((4 * (size_t)B + 255) & ~(size_t)255);
+	const size_t off_woff = 0;  // off[B]: where each Block's positions start
+	const size_t off_blocks = off_woff + ((4 * (size_t)B + 255) & ~(size_t)255);
 	const size_t off_jobs = off_blocks + ((sizeof(XzbMfBlock) * B + 255) & ~(size_t)255);
 	const size_t off_crcjobs = off_jobs + ((sizeof(XzbEncJob) * B + 255) & ~(size_t)255);
 	const size_t off_results = off_crcjobs + ((sizeof(XzbCrcJob) * B + 255) & ~(size_t)255);
@@ -820,27 +859,27 @@ static int encode_wave(xzb_ctx *ctx, const uint8_t *d_in, uint64_t in_bytes, boo
 	const size_t off_crcv = off_pend + ((4 * (size_t)B + 255) & ~(size_t)255);
 	const size_t off_ovftop = off_crcv + ((32 * (size_t)B + 255) & ~(size_t)255);  // Check field bytes, 32 per block
 	const size_t off_misc = off_ovftop + ((4 * (size_t)B + 255) & ~(size_t)255);  // [0] num_runs, [1] work counter, [2] err
-	const size_t small_size = off_misc + 256;
+	const size_t off_tiles = off_misc + 256;  // tile_block[ntiles]
+	const size_t small_size = off_tiles + 4 * (size_t)ntiles + 256;
 	EN(ctx->small, small_size);
 	uint8_t *sm = (uint8_t *)ctx->small.p;
 	std::vector<uint8_t> h_small(small_size, 0);
-	uint32_t *h_sizes = (uint32_t *)(h_small.data() + off_sizes);
+	uint32_t *h_woff = (uint32_t *)(h_small.data() + off_woff);
 	XzbMfBlock *h_blocks = (XzbMfBlock *)(h_small.data() + off_blocks);
 	XzbEncJob *h_jobs = (XzbEncJob *)(h_small.data() + off_jobs);
 	XzbCrcJob *h_crcjobs = (XzbCrcJob *)(h_small.data() + off_crcjobs);
-	const uint64_t bound = xzbi_block_bound(block_size_opt);
-	const uint32_t header_size = xzb_block_header_size(bound, block_size_opt, P.ff_len);
-	if (oneshot && B != 1) return set_err(ctx, XZB_PROG_ERROR, "one-shot framing takes exactly one block");
+	uint32_t *h_tiles = (uint32_t *)(h_small.data() + off_tiles);
 	uint64_t n_valid = 0, n_pos = 0;
 	for (uint32_t b = 0; b < B; ++b) {
-		const uint64_t off = (uint64_t)b * bs;
-		const uint32_t n = (uint32_t)std::min<uint64_t>(bs, in_bytes - off);
-		h_sizes[b] = n;
+		const size_t off = h_off[b];
+		const uint32_t n = wb[b].n;
+		h_woff[b] = h_off[b];
+		for (uint32_t t = h_off[b] / XZB_WAVE_ALIGN; t < (h_off[b] + xzb_wave_pad(n)) / XZB_WAVE_ALIGN; ++t) h_tiles[t] = b;
 		n_pos += n;
 		n_valid += n >= P.hash_bytes ? n - P.hash_bytes + 1 : 0;
 		XzbMfBlock &mb = h_blocks[b];
-		mb.buf = d_work + off; mb.n = n;
-		mb.room = (b + 1 < B || has_slack) ? n + 8 : n;
+		mb.buf = d_work + wb[b].in_off; mb.n = n;
+		mb.room = wb[b].room;
 		mb.prev2 = (const uint32_t *)ctx->prev2.p + off; mb.prev3 = (const uint32_t *)ctx->prev3.p + off;
 		mb.prevm = (const uint32_t *)ctx->prevm.p + off;
 		mb.son = (uint32_t *)ctx->son.p + 2 * off;
@@ -850,17 +889,14 @@ static int encode_wave(xzb_ctx *ctx, const uint8_t *d_in, uint64_t in_bytes, boo
 		mb.ovf_top = (uint32_t *)(sm + off_ovftop) + b;
 		mb.ovf_cap = n;
 		mb.err = (uint32_t *)(sm + off_misc) + 2;
-		h_jobs[b].in = d_in + off; h_jobs[b].in_size = n;
-		h_jobs[b].out = (uint8_t *)ctx->scratch.p + (size_t)b * scap; h_jobs[b].out_cap = scap;
-		h_jobs[b].header_size = header_size; h_jobs[b].oneshot = 0; h_jobs[b].fit_limit = bound;
-		if (oneshot) {  // block_encode_normal(), block_buffer_encoder.c:165-183
-			h_jobs[b].header_size = xzb_block_header_size(xzb_lzma2_bound(n), n, P.ff_len);
-			h_jobs[b].oneshot = 1; h_jobs[b].fit_limit = h_jobs[b].header_size + xzb_lzma2_bound(n);
-		}
-		h_crcjobs[b].data = d_in + off; h_crcjobs[b].size = n;
+		h_jobs[b].in = d_in + wb[b].in_off; h_jobs[b].in_size = n;
+		h_jobs[b].out = (uint8_t *)ctx->scratch.p + scratch_off[b]; h_jobs[b].out_cap = wb[b].scap;
+		h_jobs[b].header_size = wb[b].header_size; h_jobs[b].oneshot = wb[b].oneshot; h_jobs[b].fit_limit = wb[b].fit_limit;
+		h_crcjobs[b].data = d_in + wb[b].in_off; h_crcjobs[b].size = n;
 	}
 	CK(cudaMemcpyAsync(sm, h_small.data(), small_size, cudaMemcpyHostToDevice, st));
-	const uint32_t *d_sizes = (const uint32_t *)(sm + off_sizes);
+	const uint32_t *d_woff = (const uint32_t *)(sm + off_woff);
+	const uint32_t *d_tiles = (const uint32_t *)(sm + off_tiles);
 	const XzbMfBlock *d_blocks = (const XzbMfBlock *)(sm + off_blocks);
 	const XzbEncJob *d_jobs = (const XzbEncJob *)(sm + off_jobs);
 	const XzbCrcJob *d_crcjobs = (const XzbCrcJob *)(sm + off_crcjobs);
@@ -874,23 +910,20 @@ static int encode_wave(xzb_ctx *ctx, const uint8_t *d_in, uint64_t in_bytes, boo
 	uint64_t launches = 0;
 
 	CK(cudaEventRecord(ctx->ev[0], st));
-	{
-		dim3 grid((bs + 255) / 256, B);
-		xzb_k_hash_keys<<<grid, 256, 0, st>>>(d_work, bs, B, d_sizes, P, ctx->d_crc32, hbm, keys_a, (uint32_t *)ctx->keys_2.p,
-				(uint32_t *)ctx->keys_3.p, vals_a, (uint32_t *)ctx->mh.p);
-		++launches;
-	}
+	xzb_k_hash_keys<<<ntiles, 256, 0, st>>>(d_blocks, d_tiles, d_woff, B, P, ctx->d_crc32, hbm, keys_a, (uint32_t *)ctx->keys_2.p,
+			(uint32_t *)ctx->keys_3.p, vals_a, (uint32_t *)ctx->mh.p);
+	++launches;
 	const uint32_t pgrid = (uint32_t)((N + 255) / 256);
 	size_t tb = ctx->cub_tmp.cap;
 	if (P.hash_bytes >= 3) {
 		CK(cub::DeviceRadixSort::SortPairs(ctx->cub_tmp.p, tb, (const uint32_t *)ctx->keys_2.p, keys_b, vals_a, vals_b, (int64_t)N, 0, (int)kbits_2, st));
-		xzb_k_prev<<<pgrid, 256, 0, st>>>(keys_b, vals_b, N, 10, B, bs, (uint32_t *)ctx->prev2.p);
+		xzb_k_prev<<<pgrid, 256, 0, st>>>(keys_b, vals_b, N, 10, B, d_woff, (uint32_t *)ctx->prev2.p);
 		launches += 4;
 	}
 	if (P.hash_bytes >= 4) {
 		tb = ctx->cub_tmp.cap;
 		CK(cub::DeviceRadixSort::SortPairs(ctx->cub_tmp.p, tb, (const uint32_t *)ctx->keys_3.p, keys_b, vals_a, vals_b, (int64_t)N, 0, (int)kbits_3, st));
-		xzb_k_prev<<<pgrid, 256, 0, st>>>(keys_b, vals_b, N, 16, B, bs, (uint32_t *)ctx->prev3.p);
+		xzb_k_prev<<<pgrid, 256, 0, st>>>(keys_b, vals_b, N, 16, B, d_woff, (uint32_t *)ctx->prev3.p);
 		launches += 5;
 	}
 	tb = ctx->cub_tmp.cap;
@@ -911,7 +944,7 @@ static int encode_wave(xzb_ctx *ctx, const uint8_t *d_in, uint64_t in_bytes, boo
 	const bool overlap = ctx->overlap && P.is_bt && B <= (uint32_t)ctx->sm_count;
 	cudaStream_t st_mf = overlap ? ctx->stream_mf : st;
 	if (!P.is_bt) {
-		xzb_k_prev<<<pgrid, 256, 0, st>>>(keys_b, vals_b, N, hbm, B, bs, (uint32_t *)ctx->prevm.p);
+		xzb_k_prev<<<pgrid, 256, 0, st>>>(keys_b, vals_b, N, hbm, B, d_woff, (uint32_t *)ctx->prevm.p);
 		++launches;
 	} else {
 		XzbRunStartOp op{ keys_b, vals_b, B << hbm, seg_shift };
@@ -960,8 +993,7 @@ static int encode_wave(xzb_ctx *ctx, const uint8_t *d_in, uint64_t in_bytes, boo
 		++launches;
 	};
 	if (!P.is_bt) {
-		dim3 grid((bs + 127) / 128, B);
-		xzb_k_hc<<<grid, 128, 0, st>>>(d_blocks, P);
+		xzb_k_hc<<<2 * ntiles, 128, 0, st>>>(d_blocks, d_tiles, d_woff, P);
 		++launches;
 		CK(cudaEventRecord(ctx->ev[2], st));
 		if (check == 10) { xzb_k_sha256<<<B, 32, 0, st>>>(d_crcjobs, (uint8_t *)d_crcv); ++launches; }
@@ -1046,38 +1078,43 @@ static int encode_wave(xzb_ctx *ctx, const uint8_t *d_in, uint64_t in_bytes, boo
 	return XZB_OK;
 }
 
-static uint32_t pick_wave_blocks(xzb_ctx *ctx, uint64_t bs, const XzbParams &P, uint64_t nblocks, uint64_t reserve)
+// Device memory an encode wave may take: 85 % of what is free, counting the workspace this context already holds,
+// less `reserve`.
+static uint64_t wave_budget(xzb_ctx *ctx, uint64_t reserve)
 {
 	size_t free_b = 0, total_b = 0;
 	cudaMemGetInfo(&free_b, &total_b);
-	// memory already held by our own workspace is reusable
 	uint64_t held = 0;
 	const DevBuf *bufs[] = { &ctx->keys_a, &ctx->keys_b, &ctx->vals_a, &ctx->vals_b, &ctx->keys_2, &ctx->keys_3, &ctx->prev2, &ctx->prev3,
 		&ctx->prevm, &ctx->son, &ctx->mh, &ctx->mp, &ctx->ovf, &ctx->cub_tmp, &ctx->run_start, &ctx->run_len, &ctx->run_start_s,
 		&ctx->run_len_s, &ctx->encs, &ctx->scratch };
 	for (const DevBuf *b : bufs) held += b->cap;
-	uint64_t budget = (uint64_t)((free_b + held) * 0.85);
-	budget = budget > reserve ? budget - reserve : 0;
+	const uint64_t budget = (uint64_t)((free_b + held) * 0.85);
+	return budget > reserve ? budget - reserve : 0;
+}
+
+static uint32_t pick_wave_blocks(xzb_ctx *ctx, uint64_t bs, const XzbParams &P, uint64_t nblocks, uint64_t reserve)
+{
+	const uint64_t budget = wave_budget(ctx, reserve);
 	uint64_t per = wave_bytes_per_block(bs, P) + (P.is_bt ? 16 * bs : 0);
 	uint64_t w = per ? budget / per : 1;
 	const uint32_t hbm = bit_length(P.hash_mask);
 	const uint64_t key_cap = (1ull << (32 - hbm)) - 1;  // (B << hbm) must fit 32 bits
 	w = std::min<uint64_t>(w, key_cap);
-	w = std::min<uint64_t>(w, 0xFFFFFFF0ull / bs - 1);
+	w = std::min<uint64_t>(w, 0xFFFFFFF0ull / xzb_wave_pad(bs) - 1);
 	w = std::min<uint64_t>(w, nblocks);
 	if (ctx->max_wave_blocks) w = std::min<uint64_t>(w, ctx->max_wave_blocks);  // XZB_MAX_WAVE_BLOCKS (tests: force several waves)
 	return (uint32_t)std::max<uint64_t>(w, 1);
 }
 
-static int encode_common(xzb_ctx *ctx, const uint8_t *in, bool in_is_device, uint64_t in_size, const xzb_lzma_options *opt, uint32_t check,
-		uint64_t block_size, uint8_t *out, bool out_is_device, uint64_t out_cap, uint64_t *out_size, xzb_index_record *records,
-		bool whole_stream, bool oneshot = false)
+// Starts an encode call: clears the call's stats and error, derives the coder parameters from the options and the
+// context's filter chain, and checks the Check ID.
+static int encode_begin(xzb_ctx *ctx, const xzb_lzma_options *opt, uint32_t check, XzbParams &P)
 {
 	cudaSetDevice(ctx->device);
 	memset(&ctx->stats, 0, sizeof(ctx->stats));
 	ctx->err[0] = 0;
-	XzbParams P;
-	int r = xzb_make_params((const XzbLzmaOptions *)opt, &P);
+	const int r = xzb_make_params((const XzbLzmaOptions *)opt, &P);
 	if (r != XZB_OK) return set_err(ctx, r, "unsupported LZMA2 options");
 	if (!ctx->pre.empty()) {
 		// Filter Flags of the filters in front of LZMA2: ID, size of properties, properties (filter_flags_encoder.c:31-56;
@@ -1091,7 +1128,38 @@ static int encode_common(xzb_ctx *ctx, const uint8_t *in, bool in_is_device, uin
 		P.n_pre = (uint8_t)ctx->pre.size();
 	}
 	if (xzb_check_size(check) == 0xFFFFFFFFu) return set_err(ctx, XZB_UNSUPPORTED_CHECK, "check %u not supported", check);
-	if (oneshot) block_size = std::max<uint64_t>(in_size, 1);  // ONE Block over the whole input (stream_buffer_encoder.c:93-95)
+	return XZB_OK;
+}
+
+// Places finished Blocks (and, for framed jobs, whole one-shot Streams) with one xzb_k_pack_streams launch, then
+// synchronises.  host_out == nullptr: every job's dst is a device address.  Otherwise each dst is an offset into a
+// staging area of stage_bytes, which comes back to host_out with one copy.
+static int place_blocks(xzb_ctx *ctx, std::vector<XzbPackJob> &jobs, uint32_t check, uint8_t *host_out, size_t stage_bytes)
+{
+	cudaStream_t st = ctx->stream;
+	if (!jobs.empty()) {
+		if (host_out != nullptr) {
+			EN(ctx->out_stage, stage_bytes + 64);
+			for (XzbPackJob &j : jobs) j.dst = (uint8_t *)ctx->out_stage.p + (size_t)j.dst;
+		}
+		EN(ctx->pack_jobs, sizeof(XzbPackJob) * jobs.size());
+		CK(cudaMemcpyAsync(ctx->pack_jobs.p, jobs.data(), sizeof(XzbPackJob) * jobs.size(), cudaMemcpyHostToDevice, st));
+		xzb_k_pack_streams<<<(uint32_t)jobs.size(), 256, 0, st>>>((const XzbPackJob *)ctx->pack_jobs.p, ctx->d_crc32, check);
+		++ctx->stats.gpu_launches;
+		if (host_out != nullptr && stage_bytes > 0) CK(cudaMemcpyAsync(host_out, ctx->out_stage.p, stage_bytes, cudaMemcpyDeviceToHost, st));
+	}
+	CK(cudaStreamSynchronize(st));   // also: `jobs` is the source of the copy above
+	CK(cudaGetLastError());
+	return XZB_OK;
+}
+
+static int encode_common(xzb_ctx *ctx, const uint8_t *in, bool in_is_device, uint64_t in_size, const xzb_lzma_options *opt, uint32_t check,
+		uint64_t block_size, uint8_t *out, bool out_is_device, uint64_t out_cap, uint64_t *out_size, xzb_index_record *records,
+		bool whole_stream)
+{
+	XzbParams P;
+	int r = encode_begin(ctx, opt, check, P);
+	if (r != XZB_OK) return r;
 	if (block_size == 0) block_size = std::max<uint64_t>((uint64_t)P.dict_size * 3, 1u << 20);  // lzma_lzma2_block_size, lzma2_encoder.c:403-413
 	if (block_size > (1ull << 30)) return set_err(ctx, XZB_OPTIONS_ERROR, "block_size > 1 GiB is not supported on the GPU path");
 	const uint64_t nblocks = (in_size + block_size - 1) / block_size;
@@ -1108,9 +1176,11 @@ static int encode_common(xzb_ctx *ctx, const uint8_t *in, bool in_is_device, uin
 		pos = 12;
 	}
 	uint64_t done = 0;
-	const uint32_t scap = scratch_cap_for(block_size);
+	const uint64_t bound = xzbi_block_bound(block_size);
+	const uint32_t header_size = xzb_block_header_size(bound, block_size, P.ff_len);
 	while (done < nblocks) {
-		const uint32_t W = pick_wave_blocks(ctx, bs, P, nblocks - done, in_is_device ? 0 : (uint64_t)bs * std::min<uint64_t>(nblocks - done, 256));
+		const uint64_t stage = (uint64_t)bs * std::min<uint64_t>(nblocks - done, 256);
+		const uint32_t W = pick_wave_blocks(ctx, bs, P, nblocks - done, (in_is_device ? 0 : stage) + (out_is_device ? 0 : stage));
 		const uint64_t off = done * block_size;
 		const uint64_t wave_bytes = std::min<uint64_t>((uint64_t)W * bs, in_size - off);
 		const uint8_t *d_wave;
@@ -1123,21 +1193,32 @@ static int encode_common(xzb_ctx *ctx, const uint8_t *in, bool in_is_device, uin
 			CK(cudaEventRecord(ctx->ev[9], st));
 			d_wave = (const uint8_t *)ctx->in_stage.p;
 		}
+		const bool has_slack = !in_is_device || off + wave_bytes < in_size;
+		std::vector<XzbWaveBlock> wb(W);
+		for (uint32_t b = 0; b < W; ++b) {
+			const uint32_t n = (uint32_t)std::min<uint64_t>(bs, wave_bytes - (uint64_t)b * bs);
+			wb[b] = XzbWaveBlock{ (uint64_t)b * bs, n, (b + 1 < W || has_slack) ? n + 8 : n, header_size, 0, bound, xzb_scratch_cap(block_size) };
+		}
 		std::vector<XzbBlockResult> results;
-		r = encode_wave(ctx, d_wave, wave_bytes, !in_is_device || off + wave_bytes < in_size, W, bs, P, check, block_size, oneshot, results);
+		std::vector<size_t> sc_off;
+		r = encode_wave(ctx, d_wave, wave_bytes, wb, P, check, results, sc_off);
 		if (r != XZB_OK) return r;
 		if (!in_is_device) ctx->stats.ms_h2d += ev_ms(ctx->ev[8], ctx->ev[9]);
 		CK(cudaEventRecord(ctx->ev[10], st));
+		const uint64_t pos0 = pos;
+		std::vector<XzbPackJob> jobs(W);
 		for (uint32_t b = 0; b < W; ++b) {
 			const XzbBlockResult &res = results[b];
 			if (res.ret != XZB_OK) return set_err(ctx, (int)res.ret, "block %llu failed", (unsigned long long)(done + b));
 			if (pos + res.total_size > out_cap) return set_err(ctx, XZB_BUF_ERROR, "output buffer too small");
-			const uint8_t *src = (const uint8_t *)ctx->scratch.p + (size_t)b * scap;
-			CK(cudaMemcpyAsync(out + pos, src, res.total_size, out_is_device ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, st));
+			uint8_t *dst = out_is_device ? out + pos : (uint8_t *)(uintptr_t)(pos - pos0);
+			jobs[b] = XzbPackJob{ (const uint8_t *)ctx->scratch.p + sc_off[b], dst, 0, 0, res.total_size, 0 };
 			pos += res.total_size;
 			recs[done + b].unpadded_size = res.unpadded_size;
-			recs[done + b].uncompressed_size = std::min<uint64_t>(block_size, in_size - (done + b) * block_size);
+			recs[done + b].uncompressed_size = wb[b].n;
 		}
+		r = place_blocks(ctx, jobs, check, out_is_device ? nullptr : out + pos0, pos - pos0);
+		if (r != XZB_OK) return r;
 		CK(cudaEventRecord(ctx->ev[11], st));
 		CK(cudaStreamSynchronize(st));
 		if (!out_is_device) ctx->stats.ms_d2h += ev_ms(ctx->ev[10], ctx->ev[11]); else ctx->stats.ms_other += ev_ms(ctx->ev[10], ctx->ev[11]);
@@ -1207,16 +1288,127 @@ extern "C" uint64_t xzb_stream_buffer_bound(uint64_t in_size)
 	return bb + hb;
 }
 
+// n independent one-shot Streams.  The items are encoded in waves of similar sizes (xzb_plan_waves), each Block framed
+// as lzma_block_buffer_encode() does (block_encode_normal(), block_buffer_encoder.c:165-183: header sized from
+// lzma2_bound(n), the LZMA2 data alone must fit) and turned into its Stream by xzb_k_pack_streams.
+static int encode_batch(xzb_ctx *ctx, uint32_t n, const uint8_t *in, bool in_is_device, const uint64_t *in_off, const uint64_t *in_size,
+		const xzb_lzma_options *opt, uint32_t check, uint8_t *out, bool out_is_device, const uint64_t *out_off, const uint64_t *out_cap,
+		uint64_t *out_size, uint32_t *ret)
+{
+	XzbParams P;
+	int r = encode_begin(ctx, opt, check, P);
+	if (r != XZB_OK) return r;
+	cudaStream_t st = ctx->stream;
+	CK(cudaEventRecord(ctx->ev[6], st));
+	std::vector<uint32_t> items;       // the items with a Block
+	std::vector<uint64_t> sizes;
+	std::vector<XzbPackJob> empties;   // Streams with no Block
+	std::vector<uint32_t> empty_items;
+	for (uint32_t i = 0; i < n; ++i) {
+		out_size[i] = 0; ret[i] = XZB_OK;
+		if (in_size[i] > (1ull << 30)) { ret[i] = XZB_OPTIONS_ERROR; set_err(ctx, XZB_OPTIONS_ERROR, "block_size > 1 GiB is not supported on the GPU path"); }
+		else if (in_size[i] == 0) { empty_items.push_back(i); }
+		else { items.push_back(i); sizes.push_back(in_size[i]); }
+	}
+	// Host output goes through a staging area packed in call order of the items that fit, then back in one copy.
+	std::vector<uint8_t> host_stage;
+	auto place = [&](const std::vector<uint32_t> &who, std::vector<XzbPackJob> &jobs) -> int {
+		uint64_t stage = 0;
+		std::vector<XzbPackJob> keep;
+		std::vector<uint32_t> kept;
+		for (size_t k = 0; k < jobs.size(); ++k) {
+			const uint32_t i = who[k];
+			const uint64_t size = xzb_oneshot_stream_size(jobs[k].size, jobs[k].unpadded, jobs[k].uncomp);
+			if (size > out_cap[i]) { ret[i] = XZB_BUF_ERROR; set_err(ctx, XZB_BUF_ERROR, "output buffer too small"); continue; }
+			out_size[i] = size;
+			jobs[k].dst = out_is_device ? out + out_off[i] : (uint8_t *)(uintptr_t)stage;
+			stage += (size + 15) & ~15ull;
+			keep.push_back(jobs[k]); kept.push_back(i);
+		}
+		if (!out_is_device) host_stage.resize(stage);
+		const int pr = place_blocks(ctx, keep, check, out_is_device ? nullptr : host_stage.data(), stage);
+		if (pr != XZB_OK) return pr;
+		if (!out_is_device)
+			for (size_t k = 0; k < keep.size(); ++k)
+				memcpy(out + out_off[kept[k]], host_stage.data() + (keep[k].dst - (uint8_t *)ctx->out_stage.p), out_size[kept[k]]);
+		return XZB_OK;
+	};
+	const uint32_t hbm = bit_length(P.hash_mask);
+	std::vector<uint32_t> order, wave_start;
+	xzb_plan_waves(sizes.data(), (uint32_t)sizes.size(), xzb_wave_cost(P), wave_budget(ctx, 0), hbm, ctx->max_wave_blocks, &order, &wave_start);
+	for (size_t w = 0; w + 1 < wave_start.size(); ++w) {
+		const uint32_t B = wave_start[w + 1] - wave_start[w];
+		std::vector<uint32_t> who(B), wn(B), woff(B);
+		for (uint32_t b = 0; b < B; ++b) { who[b] = items[order[wave_start[w] + b]]; wn[b] = (uint32_t)in_size[who[b]]; }
+		// the wave's inputs side by side in HBM, each at its Block's workspace offset; the 64 bytes behind the last one
+		// are the slack the match finder may read past every Block
+		const uint64_t total = xzb_wave_offsets(wn.data(), B, woff.data());
+		EN(ctx->in_stage, total + 64);
+		uint8_t *d_wave = (uint8_t *)ctx->in_stage.p;
+		CK(cudaEventRecord(ctx->ev[8], st));
+		for (uint32_t b = 0; b < B; ++b)
+			CK(cudaMemcpyAsync(d_wave + woff[b], in + in_off[who[b]], wn[b], in_is_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, st));
+		CK(cudaEventRecord(ctx->ev[9], st));
+		std::vector<XzbWaveBlock> wb(B);
+		for (uint32_t b = 0; b < B; ++b) {
+			const uint32_t hs = xzb_block_header_size(xzb_lzma2_bound(wn[b]), wn[b], P.ff_len);
+			wb[b] = XzbWaveBlock{ woff[b], wn[b], wn[b] + 8, hs, 1, hs + xzb_lzma2_bound(wn[b]), xzb_scratch_cap(wn[b]) };
+		}
+		std::vector<XzbBlockResult> results;
+		std::vector<size_t> sc_off;
+		r = encode_wave(ctx, d_wave, total, wb, P, check, results, sc_off);
+		if (r != XZB_OK) return r;
+		ctx->stats.ms_h2d += ev_ms(ctx->ev[8], ctx->ev[9]);
+		std::vector<XzbPackJob> jobs;
+		std::vector<uint32_t> placed;
+		for (uint32_t b = 0; b < B; ++b) {
+			const XzbBlockResult &res = results[b];
+			if (res.ret != XZB_OK) { ret[who[b]] = res.ret; set_err(ctx, (int)res.ret, "item %u failed", who[b]); continue; }
+			jobs.push_back(XzbPackJob{ (const uint8_t *)ctx->scratch.p + sc_off[b], nullptr, res.unpadded_size, wn[b], res.total_size, 1 });
+			placed.push_back(who[b]);
+		}
+		r = place(placed, jobs);
+		if (r != XZB_OK) return r;
+	}
+	for (size_t k = 0; k < empty_items.size(); ++k) empties.push_back(XzbPackJob{ nullptr, nullptr, 0, 0, 0, 1 });
+	r = place(empty_items, empties);
+	if (r != XZB_OK) return r;
+	CK(cudaEventRecord(ctx->ev[7], st));
+	CK(cudaStreamSynchronize(st));
+	ctx->stats.ms_total = ev_ms(ctx->ev[6], ctx->ev[7]);
+	return XZB_OK;
+}
+
+extern "C" int xzb_stream_buffer_encode_batch(xzb_ctx *ctx, uint32_t n, const uint8_t *in, const uint64_t *in_off, const uint64_t *in_size,
+		const xzb_lzma_options *opt, uint32_t check, uint8_t *out, const uint64_t *out_off, const uint64_t *out_cap, uint64_t *out_size, uint32_t *ret)
+{
+	return encode_batch(ctx, n, in, false, in_off, in_size, opt, check, out, false, out_off, out_cap, out_size, ret);
+}
+
+extern "C" int xzb_stream_buffer_encode_batch_device(xzb_ctx *ctx, uint32_t n, const uint8_t *in, const uint64_t *in_off, const uint64_t *in_size,
+		const xzb_lzma_options *opt, uint32_t check, uint8_t *out, const uint64_t *out_off, const uint64_t *out_cap, uint64_t *out_size, uint32_t *ret)
+{
+	return encode_batch(ctx, n, in, true, in_off, in_size, opt, check, out, true, out_off, out_cap, out_size, ret);
+}
+
 extern "C" int xzb_stream_buffer_encode(xzb_ctx *ctx, const uint8_t *in, uint64_t in_size, const xzb_lzma_options *opt, uint32_t check,
 		uint8_t *out, uint64_t out_cap, uint64_t *out_size)
 {
-	return encode_common(ctx, in, false, in_size, opt, check, 0, out, false, out_cap, out_size, nullptr, true, true);
+	const uint64_t zero = 0;
+	uint64_t size = 0;
+	uint32_t ret = XZB_OK;
+	const int r = encode_batch(ctx, 1, in, false, &zero, &in_size, opt, check, out, false, &zero, &out_cap, &size, &ret);
+	if (r != XZB_OK) return r;
+	if (ret == XZB_OK) *out_size = size;
+	return (int)ret;
 }
 
 // ------------------------------------------------------------------------------------
 // Decode
 // ------------------------------------------------------------------------------------
-static int decode_batch(xzb_ctx *ctx, const std::vector<XzbDecJob> &jobs, uint32_t check, std::vector<XzbDecResult> &results, std::vector<uint64_t> &crcs,
+// Decodes the Blocks `jobs` side by side; checks[b] is the Check ID whose value crcs[b] (CRC32 / CRC64) or
+// shas[32 b ..] (SHA-256, when shas is given) receives for what Block b produced; 0 or any other ID: none.
+static int decode_batch(xzb_ctx *ctx, const std::vector<XzbDecJob> &jobs, const std::vector<uint32_t> &checks, std::vector<XzbDecResult> &results, std::vector<uint64_t> &crcs,
 		std::vector<uint8_t> *shas = nullptr, const std::vector<XzbBlockHeader> *chains = nullptr)
 {
 	cudaStream_t st = ctx->stream;
@@ -1257,23 +1449,32 @@ static int decode_batch(xzb_ctx *ctx, const std::vector<XzbDecJob> &jobs, uint32
 			ctx->stats.gpu_launches += 1;
 		}
 	}
-	if (check == 1 || check == 4) {
-		std::vector<XzbCrcJob> cj(B);
-		for (uint32_t b = 0; b < B; ++b) { cj[b].data = jobs[b].out; cj[b].size = results[b].out_used; }
-		CK(cudaMemcpyAsync(sm + off_crcjobs, cj.data(), sizeof(XzbCrcJob) * B, cudaMemcpyHostToDevice, st));
-		const bool c64 = check == 4;
-		xzb_k_crc<<<B, 1024, 0, st>>>((const XzbCrcJob *)(sm + off_crcjobs), c64 ? ctx->d_crc64 : ctx->d_crc32w, c64 ? ~0ull : 0xFFFFFFFFull, (uint64_t *)(sm + off_crcv), 1);
-		CK(cudaMemcpyAsync(crcs.data(), sm + off_crcv, 8 * (size_t)B, cudaMemcpyDeviceToHost, st));
+	// the integrity check of what each Block produced: one launch per check type over the Blocks that carry it
+	if (shas != nullptr) shas->assign(32 * (size_t)B, 0);
+	for (const uint32_t c : { 1u, 4u, 10u }) {
+		if (c == 10 && shas == nullptr) continue;
+		std::vector<XzbCrcJob> cj;
+		std::vector<uint32_t> who;
+		for (uint32_t b = 0; b < B; ++b)
+			if (checks[b] == c) { cj.push_back(XzbCrcJob{ jobs[b].out, results[b].out_used }); who.push_back(b); }
+		if (cj.empty()) continue;
+		const uint32_t nc = (uint32_t)cj.size();
+		CK(cudaMemcpyAsync(sm + off_crcjobs, cj.data(), sizeof(XzbCrcJob) * nc, cudaMemcpyHostToDevice, st));
+		std::vector<uint8_t> got(32 * (size_t)nc);
+		if (c == 10) {
+			xzb_k_sha256<<<nc, 32, 0, st>>>((const XzbCrcJob *)(sm + off_crcjobs), sm + off_crcv);
+			CK(cudaMemcpyAsync(got.data(), sm + off_crcv, 32 * (size_t)nc, cudaMemcpyDeviceToHost, st));
+		} else {
+			const bool c64 = c == 4;
+			xzb_k_crc<<<nc, 1024, 0, st>>>((const XzbCrcJob *)(sm + off_crcjobs), c64 ? ctx->d_crc64 : ctx->d_crc32w, c64 ? ~0ull : 0xFFFFFFFFull, (uint64_t *)(sm + off_crcv), 1);
+			CK(cudaMemcpyAsync(got.data(), sm + off_crcv, 8 * (size_t)nc, cudaMemcpyDeviceToHost, st));
+		}
 		ctx->stats.gpu_launches += 1;
-	}
-	if (check == 10 && shas != nullptr) {  // SHA-256 of what each block produced
-		std::vector<XzbCrcJob> cj(B);
-		for (uint32_t b = 0; b < B; ++b) { cj[b].data = jobs[b].out; cj[b].size = results[b].out_used; }
-		CK(cudaMemcpyAsync(sm + off_crcjobs, cj.data(), sizeof(XzbCrcJob) * B, cudaMemcpyHostToDevice, st));
-		xzb_k_sha256<<<B, 32, 0, st>>>((const XzbCrcJob *)(sm + off_crcjobs), sm + off_crcv);
-		shas->assign(32 * (size_t)B, 0);
-		CK(cudaMemcpyAsync(shas->data(), sm + off_crcv, 32 * (size_t)B, cudaMemcpyDeviceToHost, st));
-		ctx->stats.gpu_launches += 1;
+		CK(cudaStreamSynchronize(st));
+		for (uint32_t k = 0; k < nc; ++k) {
+			if (c == 10) memcpy(shas->data() + 32 * (size_t)who[k], got.data() + 32 * (size_t)k, 32);
+			else memcpy(&crcs[who[k]], got.data() + 8 * (size_t)k, 8);
+		}
 	}
 	CK(cudaEventRecord(ctx->ev[2], st));
 	CK(cudaStreamSynchronize(st));
@@ -1301,7 +1502,7 @@ extern "C" int xzb_decode_blocks_device(xzb_ctx *ctx, const void *d_in, const ui
 	}
 	if (check == 10 && check_out != nullptr) return set_err(ctx, XZB_UNSUPPORTED_CHECK, "check_out carries CRC values only; verify SHA-256 Streams with xzb_stream_decode*");
 	std::vector<XzbDecResult> results; std::vector<uint64_t> crcs;
-	int r = decode_batch(ctx, jobs, check, results, crcs);
+	int r = decode_batch(ctx, jobs, std::vector<uint32_t>(nblocks, check), results, crcs);
 	if (r != XZB_OK) return r;
 	for (uint32_t b = 0; b < nblocks; ++b) {
 		uint32_t code = results[b].ret;
@@ -1375,6 +1576,193 @@ extern "C" int xzb_stream_decode_flags(xzb_ctx *ctx, const uint8_t *in, uint64_t
 	return xzb_stream_decode_prior(ctx, in, in_size, out, out_cap, out_size, in_used, flags, nullptr, 0);
 }
 
+// One Stream in flight in decode_streams(): the caller's view, and the decoder's cursor over it.
+struct XzbDecStream {
+	const uint8_t *in; uint64_t in_size;     // host
+	uint8_t *out; uint64_t out_cap;          // host
+	uint32_t flags;
+	const xzb_index_record *prior; uint64_t n_prior;  // see xzb_stream_decode_prior
+	// results
+	int ret = XZB_OK;
+	int buf_reason = 1;                      // why XZB_BUF_ERROR: 1 = the input ended early, 2 = the output is too small
+	uint64_t in_used = 0, out_size = 0;
+	// cursor
+	bool done = false, at_index = false;
+	uint32_t check = 0, csize = 0;
+	bool verify = true;
+	uint64_t d_in = 0, d_out = 0;            // its input / output in ctx->dec_in / ctx->dec_out
+	uint64_t ip = 12, op = 0;
+	std::vector<xzb_index_record> recs;
+	// the Blocks of the current round
+	std::vector<XzbBlockHeader> batch;
+	std::vector<uint64_t> hdr_offs, out_offs;
+	std::vector<bool> truncated, out_exact;
+	uint64_t bip = 0;
+	int pending = XZB_OK;                    // error discovered while scanning ahead: reported after the round
+	size_t job0 = 0;
+};
+
+// Index + Stream Footer behind the last Block (common/index_hash.c:175-341, stream_decoder.c:266-332), then the
+// Stream's results.
+static void decode_stream_end(xzb_ctx *ctx, XzbDecStream &s)
+{
+	if (s.ret == XZB_OK) {
+		const XzbIndexWant want{ s.recs.data(), s.recs.size() };
+		XzbIndexRead x;
+		s.ret = xzb_index_read(ctx->h_tab.crc32, s.in + s.ip, s.in_size - s.ip, &want, &x);
+		s.ip += x.stop;
+		uint32_t fcheck = 0; uint64_t fisize = 0;
+		if (s.ret == XZB_OK && s.in_size - s.ip < 12) s.ret = XZB_BUF_ERROR;
+		if (s.ret == XZB_OK) s.ret = xzb_stream_footer_decode(ctx->h_tab.crc32, s.in + s.ip, &fcheck, &fisize);
+		if (s.ret == XZB_OK && (fisize != x.end || fcheck != s.check)) s.ret = XZB_DATA_ERROR;
+		if (s.ret == XZB_OK) s.ip += 12;
+	}
+	s.in_used = s.ip;
+	s.out_size = s.op;
+	s.done = true;
+}
+
+// Decodes the Streams S side by side.  Their inputs go to HBM in one copy of the span they cover; each round scans the
+// next run of sized Blocks of every unfinished Stream (an unsized Block gets a round of its own), decodes all of them
+// with one decode_batch (at most 4096 Blocks per launch), and validates each Stream's Blocks in Stream order.  Returns
+// XZB_OK or an error of the whole call (device); the Streams' own verdicts are in S.
+static int decode_streams(xzb_ctx *ctx, std::vector<XzbDecStream> &S)
+{
+	cudaStream_t st = ctx->stream;
+	const uint8_t *lo = nullptr, *hi = nullptr;
+	uint64_t out_total = 0;
+	for (XzbDecStream &s : S) {
+		s.recs.assign(s.prior, s.prior + s.n_prior);
+		if (s.in_size < 12) { s.ret = XZB_BUF_ERROR; s.done = true; continue; }
+		const int hr = xzb_stream_header_decode(ctx->h_tab.crc32, s.in, &s.check);
+		if (hr != XZB_OK) { s.ret = hr; s.done = true; continue; }
+		s.csize = xzb_check_field_size(s.check);
+		// Checks other than CRC32 / CRC64 / SHA-256 are reserved IDs: like the reference
+		// (block_decoder.c:178-190 compares only when lzma_check_is_supported()) they are skipped.
+		s.verify = !(s.flags & XZB_DEC_IGNORE_CHECK);  // LZMA_IGNORE_CHECK, stream_decoder.c:188-190
+		if (lo == nullptr || s.in < lo) lo = s.in;
+		if (hi == nullptr || s.in + s.in_size > hi) hi = s.in + s.in_size;
+		s.d_out = out_total;
+		out_total += (s.out_cap + 64 + 255) & ~255ull;
+	}
+	if (lo == nullptr) return XZB_OK;
+	CK(cudaEventRecord(ctx->ev[6], st));
+	EN(ctx->dec_in, (size_t)(hi - lo) + 64);
+	CK(cudaEventRecord(ctx->ev[8], st));
+	CK(cudaMemcpyAsync(ctx->dec_in.p, lo, (size_t)(hi - lo), cudaMemcpyHostToDevice, st));
+	CK(cudaEventRecord(ctx->ev[9], st));
+	const uint8_t *d_in = (const uint8_t *)ctx->dec_in.p;
+	EN(ctx->dec_out, out_total);
+	uint8_t *d_out = (uint8_t *)ctx->dec_out.p;
+	for (XzbDecStream &s : S) s.d_in = (uint64_t)(s.in - lo);
+
+	for (;;) {
+		std::vector<XzbDecJob> jobs;
+		std::vector<uint32_t> checks;
+		std::vector<XzbBlockHeader> hdrs;
+		std::vector<XzbDecStream *> round;
+		bool any_chain = false;
+		for (XzbDecStream &s : S) {
+			if (s.done || jobs.size() >= 4096) continue;
+			// gather a run of blocks whose headers carry both sizes (stream_decoder_mt.c:862-931)
+			s.batch.clear(); s.hdr_offs.clear(); s.out_offs.clear();
+			s.pending = XZB_OK;
+			s.bip = s.ip;
+			uint64_t bop = s.op;
+			for (;;) {
+				if (s.bip >= s.in_size) { s.pending = XZB_BUF_ERROR; break; }
+				if (s.in[s.bip] == 0x00) { s.at_index = true; break; }
+				XzbBlockHeader hb;
+				const int r = xzb_block_header_decode(ctx->h_tab.crc32, s.in + s.bip, s.in_size - s.bip, &hb);
+				if (r != XZB_OK) { s.pending = r; break; }
+				const bool sized = hb.comp != UINT64_MAX && hb.uncomp != UINT64_MAX;
+				if (!sized && !s.batch.empty()) break;  // decode what we have first
+				s.batch.push_back(hb); s.hdr_offs.push_back(s.bip); s.out_offs.push_back(bop);
+				if (!sized) break;  // direct mode: one block at a time
+				const uint64_t padded = (hb.comp + 3) & ~3ull;
+				if (s.in_size - (s.bip + hb.hsize) < padded + s.csize || s.out_cap - bop < hb.uncomp) break;  // let the per-block logic report it
+				s.bip += hb.hsize + padded + s.csize; bop += hb.uncomp;
+				if (jobs.size() + s.batch.size() >= 4096) break;
+			}
+			if (s.batch.empty()) { s.ret = s.pending; decode_stream_end(ctx, s); continue; }
+			s.job0 = jobs.size();
+			s.truncated.assign(s.batch.size(), true); s.out_exact.assign(s.batch.size(), false);
+			for (size_t b = 0; b < s.batch.size(); ++b) {
+				const XzbBlockHeader &hb = s.batch[b];
+				const uint64_t dpos = s.hdr_offs[b] + hb.hsize;
+				uint64_t in_avail = s.in_size - dpos;
+				if (hb.comp != UINT64_MAX && hb.comp <= in_avail) { in_avail = hb.comp; s.truncated[b] = false; }
+				uint64_t out_limit = s.out_cap - s.out_offs[b];
+				if (hb.uncomp != UINT64_MAX && hb.uncomp <= out_limit) { out_limit = hb.uncomp; s.out_exact[b] = true; }
+				if (in_avail > 0xFFFFFFF0ull || out_limit > 0xFFFFFFF0ull) { in_avail = std::min<uint64_t>(in_avail, 0xFFFFFFF0ull); out_limit = std::min<uint64_t>(out_limit, 0xFFFFFFF0ull); }
+				XzbDecJob j;
+				j.in = d_in + s.d_in + dpos; j.in_size = (uint32_t)in_avail;
+				j.out = d_out + s.d_out + s.out_offs[b]; j.out_limit = (uint32_t)out_limit; j.dict_size = hb.dict_size;
+				jobs.push_back(j);
+				checks.push_back(s.verify ? s.check : 0);
+				hdrs.push_back(hb);
+				any_chain = any_chain || hb.n_pre != 0;
+			}
+			round.push_back(&s);
+		}
+		if (jobs.empty()) break;
+		std::vector<XzbDecResult> results; std::vector<uint64_t> crcs; std::vector<uint8_t> shas;
+		int r = decode_batch(ctx, jobs, checks, results, crcs, &shas, any_chain ? &hdrs : nullptr);
+		if (r != XZB_OK) return r;
+		for (XzbDecStream *sp : round) {
+			XzbDecStream &s = *sp;
+			// per-block validation in stream order: common/block_decoder.c:64-200.  Like the reference
+			// (lz_decoder.c:128-160 copies what was decoded before it looks at the return code), the bytes a
+			// failing Block produced before the error are still delivered.
+			for (size_t b = 0; b < s.batch.size() && s.ret == XZB_OK; ++b) {
+				const XzbBlockHeader &hb = s.batch[b];
+				const size_t j = s.job0 + b;
+				const XzbDecResult &res = results[j];
+				const uint64_t op_fail = s.out_offs[b] + res.out_used;
+				int ret = XZB_OK;
+				if (res.ret == XZB_NEED_INPUT) ret = s.truncated[b] ? XZB_BUF_ERROR : XZB_DATA_ERROR;
+				else if (res.ret == XZB_NEED_OUTPUT) { ret = s.out_exact[b] ? XZB_DATA_ERROR : XZB_BUF_ERROR; s.buf_reason = 2; }
+				else if (res.ret != XZB_OK) ret = (int)res.ret;
+				else if ((hb.comp != UINT64_MAX && res.in_used != hb.comp) || (hb.uncomp != UINT64_MAX && res.out_used != hb.uncomp)) ret = XZB_DATA_ERROR;
+				uint64_t p = s.hdr_offs[b] + hb.hsize + res.in_used;
+				uint64_t c = res.in_used;
+				while (ret == XZB_OK && (c & 3)) {
+					if (p >= s.in_size) ret = XZB_BUF_ERROR;
+					else if (s.in[p++] != 0x00) ret = XZB_DATA_ERROR;
+					++c;
+				}
+				if (ret == XZB_OK && s.in_size - p < s.csize) ret = XZB_BUF_ERROR;
+				if (ret == XZB_OK && s.verify) {
+					const uint8_t *f = s.in + p;
+					if (s.check == 1) { if ((uint32_t)crcs[j] != xzb_rd32(f)) ret = XZB_DATA_ERROR; }
+					else if (s.check == 4) { if (crcs[j] != ((uint64_t)xzb_rd32(f) | ((uint64_t)xzb_rd32(f + 4) << 32))) ret = XZB_DATA_ERROR; }
+					else if (s.check == 10) { if (memcmp(shas.data() + 32 * j, f, 32) != 0) ret = XZB_DATA_ERROR; }
+				}
+				s.ret = ret;
+				if (ret != XZB_OK) { s.op = op_fail; break; }
+				p += s.csize;
+				xzb_index_record rec; rec.unpadded_size = hb.hsize + res.in_used + s.csize; rec.uncompressed_size = res.out_used;
+				s.recs.push_back(rec);
+				s.ip = p; s.op = s.out_offs[b] + res.out_used;
+				ctx->stats.n_positions += res.out_used;
+			}
+			if (s.ret == XZB_OK && s.pending != XZB_OK && s.ip == s.bip) s.ret = s.pending;
+			if (s.ret != XZB_OK || s.at_index) decode_stream_end(ctx, s);
+		}
+	}
+	// bytes of successfully validated blocks are delivered even when a later block fails
+	CK(cudaEventRecord(ctx->ev[10], st));
+	for (const XzbDecStream &s : S)
+		if (s.out_size > 0) CK(cudaMemcpyAsync(s.out, d_out + s.d_out, s.out_size, cudaMemcpyDeviceToHost, st));
+	CK(cudaEventRecord(ctx->ev[11], st));
+	CK(cudaEventRecord(ctx->ev[7], st));
+	CK(cudaStreamSynchronize(st));
+	ctx->stats.ms_h2d = ev_ms(ctx->ev[8], ctx->ev[9]);
+	ctx->stats.ms_d2h = ev_ms(ctx->ev[10], ctx->ev[11]);
+	ctx->stats.ms_total = ev_ms(ctx->ev[6], ctx->ev[7]);
+	return XZB_OK;
+}
+
 // The same with the Index records of Blocks that were already decoded (and removed from `in`) by earlier
 // calls: a caller that streams a long Stream hands its complete Blocks over in parts and gives the last
 // part -- whatever Blocks remain, the real Index and the Stream Footer -- together with the records of
@@ -1383,136 +1771,65 @@ extern "C" int xzb_stream_decode_prior(xzb_ctx *ctx, const uint8_t *in, uint64_t
 		uint64_t *in_used, uint32_t flags, const xzb_index_record *prior, uint64_t n_prior)
 {
 	*in_used = 0;
+	*out_size = 0;
 	cudaSetDevice(ctx->device);
 	memset(&ctx->stats, 0, sizeof(ctx->stats));
 	ctx->err[0] = 0;
-	*out_size = 0;
-	cudaStream_t st = ctx->stream;
 	// XZB_BUF_ERROR has two causes that the one-shot API tells apart (stream_buffer_decoder.c:56-71):
 	// 1 = the input ended early, 2 = the output buffer is too small.
 	ctx->dec_buf_reason = 1;
-	int buf_reason = 1;
-	if (in_size < 12) return XZB_BUF_ERROR;
-	uint32_t check = 0;
-	const int hr = xzb_stream_header_decode(ctx->h_tab.crc32, in, &check);
-	if (hr != XZB_OK) return hr;
-	const uint32_t csize = xzb_check_field_size(check);
-	// Checks other than CRC32 / CRC64 / SHA-256 are reserved IDs: like the reference
-	// (block_decoder.c:178-190 compares only when lzma_check_is_supported()) they are skipped.
-	const bool verify = !(flags & XZB_DEC_IGNORE_CHECK);  // LZMA_IGNORE_CHECK, stream_decoder.c:188-190
-	CK(cudaEventRecord(ctx->ev[6], st));
-	// whole input to HBM once; blocks are located by walking the headers on the host
-	EN(ctx->dec_in, in_size + 64);
-	CK(cudaEventRecord(ctx->ev[8], st));
-	CK(cudaMemcpyAsync(ctx->dec_in.p, in, in_size, cudaMemcpyHostToDevice, st));
-	CK(cudaEventRecord(ctx->ev[9], st));
-	const uint8_t *d_in = (const uint8_t *)ctx->dec_in.p;
-	EN(ctx->dec_out, out_cap + 64);
-	uint8_t *d_out = (uint8_t *)ctx->dec_out.p;
+	std::vector<XzbDecStream> S(1);
+	S[0].in = in; S[0].in_size = in_size; S[0].out = out; S[0].out_cap = out_cap; S[0].flags = flags;
+	S[0].prior = prior; S[0].n_prior = n_prior;
+	const int r = decode_streams(ctx, S);
+	if (r != XZB_OK) return r;
+	*in_used = S[0].in_used;
+	*out_size = S[0].out_size;
+	ctx->dec_buf_reason = S[0].buf_reason;
+	return S[0].ret;
+}
 
-	uint64_t ip = 12, op = 0;
-	std::vector<xzb_index_record> recs(prior, prior + n_prior);
-	int ret = XZB_OK;
-	bool at_index = false;
-	while (!at_index) {
-		// gather a batch of blocks whose headers carry both sizes (stream_decoder_mt.c:862-931)
-		std::vector<XzbBlockHeader> batch;
-		std::vector<uint64_t> hdr_offs, out_offs;
-		uint64_t bip = ip, bop = op;
-		int pending = XZB_OK;  // error discovered while scanning ahead: report after the batch
-		for (;;) {
-			if (bip >= in_size) { pending = XZB_BUF_ERROR; break; }
-			if (in[bip] == 0x00) { at_index = true; break; }
-			XzbBlockHeader hb;
-			const int r = xzb_block_header_decode(ctx->h_tab.crc32, in + bip, in_size - bip, &hb);
-			if (r != XZB_OK) { pending = r; break; }
-			const bool sized = hb.comp != UINT64_MAX && hb.uncomp != UINT64_MAX;
-			if (!sized && !batch.empty()) break;  // decode what we have first
-			batch.push_back(hb); hdr_offs.push_back(bip); out_offs.push_back(bop);
-			if (!sized) break;  // direct mode: one block at a time
-			const uint64_t padded = (hb.comp + 3) & ~3ull;
-			if (in_size - (bip + hb.hsize) < padded + csize || out_cap - bop < hb.uncomp) break;  // let the per-block logic report it
-			bip += hb.hsize + padded + csize; bop += hb.uncomp;
-			if (batch.size() >= 4096) break;
+// n independent Streams with xzb_stream_buffer_decode()'s result mapping per item.  Items go to the device in groups
+// whose inputs and output slots fit the memory budget.
+extern "C" int xzb_stream_buffer_decode_batch(xzb_ctx *ctx, uint32_t n, const uint8_t *in, const uint64_t *in_off, const uint64_t *in_size,
+		uint8_t *out, const uint64_t *out_off, const uint64_t *out_cap, uint64_t *out_size, uint64_t *in_used, uint32_t *ret, uint32_t flags)
+{
+	cudaSetDevice(ctx->device);
+	memset(&ctx->stats, 0, sizeof(ctx->stats));
+	ctx->err[0] = 0;
+	size_t free_b = 0, total_b = 0;
+	cudaMemGetInfo(&free_b, &total_b);
+	const uint64_t budget = (uint64_t)((free_b + ctx->dec_in.cap + ctx->dec_out.cap) * 0.85);
+	xzb_stats sum;
+	memset(&sum, 0, sizeof(sum));
+	for (uint32_t i0 = 0; i0 < n;) {
+		std::vector<XzbDecStream> S;
+		uint64_t lo = UINT64_MAX, hi = 0, outs = 0;
+		uint32_t i = i0;
+		for (; i < n; ++i) {
+			const uint64_t l = std::min(lo, in_off[i]), h = std::max(hi, in_off[i] + in_size[i]), o = outs + ((out_cap[i] + 64 + 255) & ~255ull);
+			if (i > i0 && (h - l) + o > budget) break;
+			lo = l; hi = h; outs = o;
+			XzbDecStream s;
+			s.in = in + in_off[i]; s.in_size = in_size[i]; s.out = out + out_off[i]; s.out_cap = out_cap[i]; s.flags = flags;
+			s.prior = nullptr; s.n_prior = 0;
+			S.push_back(std::move(s));
 		}
-		if (batch.empty()) { ret = pending; break; }
-		std::vector<XzbDecJob> jobs(batch.size());
-		std::vector<bool> truncated(batch.size()), out_exact(batch.size());
-		for (size_t b = 0; b < batch.size(); ++b) {
-			const XzbBlockHeader &hb = batch[b];
-			const uint64_t dpos = hdr_offs[b] + hb.hsize;
-			uint64_t in_avail = in_size - dpos; truncated[b] = true;
-			if (hb.comp != UINT64_MAX && hb.comp <= in_avail) { in_avail = hb.comp; truncated[b] = false; }
-			uint64_t out_limit = out_cap - out_offs[b]; out_exact[b] = false;
-			if (hb.uncomp != UINT64_MAX && hb.uncomp <= out_limit) { out_limit = hb.uncomp; out_exact[b] = true; }
-			if (in_avail > 0xFFFFFFF0ull || out_limit > 0xFFFFFFF0ull) { in_avail = std::min<uint64_t>(in_avail, 0xFFFFFFF0ull); out_limit = std::min<uint64_t>(out_limit, 0xFFFFFFF0ull); }
-			jobs[b].in = d_in + dpos; jobs[b].in_size = (uint32_t)in_avail;
-			jobs[b].out = d_out + out_offs[b]; jobs[b].out_limit = (uint32_t)out_limit; jobs[b].dict_size = hb.dict_size;
-		}
-		std::vector<XzbDecResult> results; std::vector<uint64_t> crcs; std::vector<uint8_t> shas;
-		bool any_chain = false;
-		for (const XzbBlockHeader &hb : batch) any_chain = any_chain || hb.n_pre != 0;
-		int r = decode_batch(ctx, jobs, verify ? check : 0, results, crcs, &shas, any_chain ? &batch : nullptr);
+		const int r = decode_streams(ctx, S);
 		if (r != XZB_OK) return r;
-		// per-block validation in stream order: common/block_decoder.c:64-200.  Like the reference
-		// (lz_decoder.c:128-160 copies what was decoded before it looks at the return code), the bytes a
-		// failing Block produced before the error are still delivered.
-		for (size_t b = 0; b < batch.size() && ret == XZB_OK; ++b) {
-			const XzbBlockHeader &hb = batch[b];
-			const XzbDecResult &res = results[b];
-			const uint64_t op_fail = out_offs[b] + res.out_used;
-			if (res.ret == XZB_NEED_INPUT) ret = truncated[b] ? XZB_BUF_ERROR : XZB_DATA_ERROR;
-			else if (res.ret == XZB_NEED_OUTPUT) { ret = out_exact[b] ? XZB_DATA_ERROR : XZB_BUF_ERROR; buf_reason = 2; }
-			else if (res.ret != XZB_OK) ret = (int)res.ret;
-			else if ((hb.comp != UINT64_MAX && res.in_used != hb.comp) || (hb.uncomp != UINT64_MAX && res.out_used != hb.uncomp)) ret = XZB_DATA_ERROR;
-			uint64_t p = hdr_offs[b] + hb.hsize + res.in_used;
-			uint64_t c = res.in_used;
-			while (ret == XZB_OK && (c & 3)) {
-				if (p >= in_size) ret = XZB_BUF_ERROR;
-				else if (in[p++] != 0x00) ret = XZB_DATA_ERROR;
-				++c;
-			}
-			if (ret == XZB_OK && in_size - p < csize) ret = XZB_BUF_ERROR;
-			if (ret == XZB_OK && verify) {
-				if (check == 1) { if ((uint32_t)crcs[b] != xzb_rd32(in + p)) ret = XZB_DATA_ERROR; }
-				else if (check == 4) { if (crcs[b] != ((uint64_t)xzb_rd32(in + p) | ((uint64_t)xzb_rd32(in + p + 4) << 32))) ret = XZB_DATA_ERROR; }
-				else if (check == 10) { if (memcmp(shas.data() + 32 * b, in + p, 32) != 0) ret = XZB_DATA_ERROR; }
-			}
-			if (ret != XZB_OK) { op = op_fail; break; }
-			p += csize;
-			xzb_index_record rec; rec.unpadded_size = hb.hsize + res.in_used + csize; rec.uncompressed_size = res.out_used;
-			recs.push_back(rec);
-			ip = p; op = out_offs[b] + res.out_used;
-			ctx->stats.n_positions += res.out_used;
+		for (uint32_t k = 0; k < S.size(); ++k) {
+			int code = S[k].ret;
+			if (code == XZB_BUF_ERROR && S[k].buf_reason == 1) code = XZB_DATA_ERROR;   // as xzb_stream_buffer_decode()
+			ret[i0 + k] = (uint32_t)code; out_size[i0 + k] = S[k].out_size; in_used[i0 + k] = S[k].in_used;
 		}
-		if (ret != XZB_OK) break;
-		if (pending != XZB_OK && ip == bip) { ret = pending; break; }
+		sum.ms_total += ctx->stats.ms_total; sum.ms_h2d += ctx->stats.ms_h2d; sum.ms_d2h += ctx->stats.ms_d2h;
+		sum.ms_decode += ctx->stats.ms_decode; sum.ms_other += ctx->stats.ms_other; sum.gpu_launches += ctx->stats.gpu_launches;
+		sum.n_blocks += ctx->stats.n_blocks; sum.n_positions += ctx->stats.n_positions;
+		memset(&ctx->stats, 0, sizeof(ctx->stats));
+		i0 = i;
 	}
-	if (ret == XZB_OK) {
-		// Index + Stream Footer: common/index_hash.c:175-341, stream_decoder.c:266-332
-		const XzbIndexWant want{ recs.data(), recs.size() };
-		XzbIndexRead x;
-		ret = xzb_index_read(ctx->h_tab.crc32, in + ip, in_size - ip, &want, &x);
-		ip += x.stop;
-		uint32_t fcheck = 0; uint64_t fisize = 0;
-		if (ret == XZB_OK && in_size - ip < 12) ret = XZB_BUF_ERROR;
-		if (ret == XZB_OK) ret = xzb_stream_footer_decode(ctx->h_tab.crc32, in + ip, &fcheck, &fisize);
-		if (ret == XZB_OK && (fisize != x.end || fcheck != check)) ret = XZB_DATA_ERROR;
-		if (ret == XZB_OK) ip += 12;
-	}
-	*in_used = ip;
-	ctx->dec_buf_reason = buf_reason;
-	// bytes of successfully validated blocks are delivered even when a later block fails
-	CK(cudaEventRecord(ctx->ev[10], st));
-	if (op > 0) CK(cudaMemcpyAsync(out, d_out, op, cudaMemcpyDeviceToHost, st));
-	CK(cudaEventRecord(ctx->ev[11], st));
-	CK(cudaEventRecord(ctx->ev[7], st));
-	CK(cudaStreamSynchronize(st));
-	ctx->stats.ms_h2d = ev_ms(ctx->ev[8], ctx->ev[9]);
-	ctx->stats.ms_d2h = ev_ms(ctx->ev[10], ctx->ev[11]);
-	ctx->stats.ms_total = ev_ms(ctx->ev[6], ctx->ev[7]);
-	*out_size = op;
-	return ret;
+	ctx->stats = sum;
+	return XZB_OK;
 }
 
 static_assert(sizeof(FS<false>) <= XZB_SOLO_SMEM && 2 * XZB_SOLO_SMEM > 228 * 1024 && XZB_SOLO_SMEM <= 227 * 1024,

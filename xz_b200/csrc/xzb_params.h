@@ -4,6 +4,9 @@
 // lzma/lzma_encoder_presets.c:16-63, check/crc32_tablegen.c, check/crc64_tablegen.c,
 // rangecoder/price_tablegen.c:28-56.
 #pragma once
+#include <algorithm>
+#include <vector>
+
 #include "xzb_common.cuh"
 #include "xzb_frame.cuh"
 
@@ -73,6 +76,59 @@ static inline int xzb_make_params(const XzbLzmaOptions *o, XzbParams *P)
 	P->lclppb = (uint8_t)((o->pb * 5 + o->lp) * 9 + o->lc);
 	P->n_pre = 0; P->ff_len = 0;
 	return XZB_OK;
+}
+
+// ---- wave layout and planning (host) ----
+// A wave is B Blocks resident in HBM side by side.  Block b's positions start at off[b] in every per-position array
+// (keys, prev*, son, mh, mp, ovf); each start is a multiple of XZB_WAVE_ALIGN positions, so a 256-position tile of the
+// match-finder launches belongs to exactly one Block and no cache line of mh / mp holds two Blocks' rows.
+#define XZB_WAVE_ALIGN 256u
+
+static inline uint64_t xzb_wave_pad(uint64_t n) { return (n + XZB_WAVE_ALIGN - 1) & ~(uint64_t)(XZB_WAVE_ALIGN - 1); }
+
+// Scratch a Block of n bytes is coded into (header + LZMA2 data + padding + check, with room to spare).
+static inline uint32_t xzb_scratch_cap(uint64_t n) { return (uint32_t)(n + n / 4096 + 70000 + 1024) & ~15u; }
+
+// Workspace of one Block: per_byte for each (padded) position, per_block on top of that.
+struct XzbWaveCost { uint64_t per_byte, per_block; };
+static inline XzbWaveCost xzb_wave_cost(const XzbParams &P)
+{
+	// keys, vals (two each), prev2/3/m, mh, ovf, mp; BT adds son and the run lists; scratch; in- and output staging
+	const uint64_t per_byte = 16 + 8 + 12 + 8 + 4 + 8 * (uint64_t)P.mstride + 8 + (P.is_bt ? 16 : 0) + 2 + 2;
+	return XzbWaveCost{ per_byte, 70000 + 1024 + 4096 + 256 };
+}
+
+// Batch wave planner.  Items (sizes[i] > 0) are taken largest first (ties in index order), so a wave holds similar
+// sizes and its longest serial chains are dispatched first; a wave takes items while all of these hold:
+//   cost.per_byte * sum(padded n) + cost.per_block * B <= budget  (a wave always takes at least one item),
+//   (B << hash_bits) < 2^32  (the sort keys are (block << hash_bits) | hash),
+//   sum(padded n) < 2^32 - 16,  B <= max_blocks (0: no limit).
+// order: item indices in wave order; wave_start: index into `order` where each wave begins, plus order.size().
+static inline void xzb_plan_waves(const uint64_t *sizes, uint32_t n, XzbWaveCost cost, uint64_t budget, uint32_t hash_bits,
+		uint32_t max_blocks, std::vector<uint32_t> *order, std::vector<uint32_t> *wave_start)
+{
+	order->resize(n);
+	for (uint32_t i = 0; i < n; ++i) (*order)[i] = i;
+	std::stable_sort(order->begin(), order->end(), [&](uint32_t a, uint32_t b) { return sizes[a] > sizes[b]; });
+	const uint64_t key_cap = (1ull << (32 - hash_bits)) - 1;
+	wave_start->clear();
+	uint64_t B = 0, pos = 0;
+	for (uint32_t k = 0; k < n; ++k) {
+		const uint64_t np = xzb_wave_pad(sizes[(*order)[k]]);
+		const bool fits = B > 0 && B + 1 <= key_cap && (max_blocks == 0 || B + 1 <= max_blocks) && pos + np < 0xFFFFFFF0ull
+			&& cost.per_byte * (pos + np) + cost.per_block * (B + 1) <= budget;
+		if (!fits) { wave_start->push_back(k); B = 0; pos = 0; }
+		++B; pos += np;
+	}
+	wave_start->push_back(n);
+}
+
+// Start of each Block's positions in a wave of Blocks of sizes n[0..B): the padded sizes summed.  Returns the total.
+static inline uint64_t xzb_wave_offsets(const uint32_t *n, uint32_t B, uint32_t *off)
+{
+	uint64_t pos = 0;
+	for (uint32_t b = 0; b < B; ++b) { off[b] = (uint32_t)pos; pos += xzb_wave_pad(n[b]); }
+	return pos;
 }
 
 struct XzbHostTables { uint32_t crc32[256]; uint64_t crc64[256]; uint8_t prices[128]; };
