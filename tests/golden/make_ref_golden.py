@@ -3,7 +3,8 @@
 (oracle/_ref, built by oracle/Makefile.ref where the reference tree exists).
 
 The reference's answers on the tests' seeded inputs (filters, encoders, decoder verdicts, the <lzma.h>
-struct layout, `xz -6 -T1` Streams), stored as the first 48 bits of SHA-256.
+struct layout, `xz -6 -T1` Streams, the LZMA2 option sweep of test_gpu_option_sweep.py and its Streams with rewritten
+dictionary sizes), stored as the first 48 bits of SHA-256.
 """
 import ctypes as C
 import json
@@ -19,6 +20,7 @@ import xzlibs as X
 import test_api_cpu as API
 import test_filters_cpu as F
 import test_gpu_filters as G
+import test_gpu_option_sweep as S
 import test_oracle as O
 
 sys.path.insert(0, os.path.dirname(TESTS))
@@ -50,6 +52,29 @@ def ref_chain_encode(data, chain, preset, bs, check=4):
     return bytes(out[:sz.value])
 
 
+def opt_sweep():
+    """lzma_stream_encoder_mt with each sweep case's LZMA2 options."""
+    out = {}
+    for c in S.sweep_cases():
+        threads = 1 if c.opts.dict_size >= 64 * S.MiB else 0   # about 0.6 GiB of match finder per thread at 64 MiB
+        out[S.key(c)] = sha(X.ref_encode(c.data, len(c.data), 0, c.block_size, c.check, threads=threads, opts=c.opts))
+    return out
+
+
+def dict_header():
+    """The single-threaded decoder's [ret, out_size, output] on Streams whose Block Headers announce each dictionary
+    size property (and invalid ones)."""
+    out = {}
+    for name, o, bs, data in S.dict_header_streams():
+        xz = X.ref_encode(data, len(data), 0, bs, opts=o)
+        props = {}
+        for prop in S.DICT_PROPS:
+            r, back = X.ref_decode(S.set_dict_prop(xz, prop), len(data))
+            props[str(prop)] = [r, len(back), sha(back)]
+        out[name] = {"stream": sha(xz), "props": props}
+    return out
+
+
 def main():
     assert X.have_ref(), "oracle/_ref is not built"
     assert REF and os.path.isdir(REF), "the reference source tree is not there (XZ_REFERENCE)"
@@ -78,6 +103,8 @@ def main():
     buf = X.gendata("T", 300000)
     for o in O.mf_options():
         g["mf_encode"][O.mf_key(o)] = sha(X.ref_encode(buf, 300000, 0, 1 << 20, opts=o))
+    g["opt_sweep"] = opt_sweep()
+    g["dict_header"] = dict_header()
     with tempfile.TemporaryDirectory() as d:
         src = os.path.join(d, "l.c")
         open(src, "w").write(API.LAYOUT_PROG.replace("HEADER", "<lzma.h>"))
