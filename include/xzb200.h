@@ -203,6 +203,19 @@ int xzb_stream_buffer_decode(xzb_ctx *ctx, const uint8_t *in, uint64_t in_size,
 int xzb_stream_buffer_decode_batch(xzb_ctx *ctx, uint32_t n, const uint8_t *in, const uint64_t *in_off,
 		const uint64_t *in_size, uint8_t *out, const uint64_t *out_off, const uint64_t *out_cap,
 		uint64_t *out_size, uint64_t *in_used, uint32_t *ret, uint32_t flags);
+/* The same with `d_in` and `d_out` in device memory (the offset, size and result arrays stay on the host).  The
+ * container (Stream Header, Block Headers, padding, Check fields, Index, Stream Footer) is read on the GPU and each
+ * Block decodes straight into its item's slot: no item data crosses PCIe, only per-item results and a few counters.
+ *   - Per item, (ret, out_size, in_used) == xzb_stream_buffer_decode_batch() for the same bytes, out_cap and flags
+ *     (XZB_DATA_ERROR for input that ends early, XZB_BUF_ERROR for a slot that is too small, XZB_DEC_IGNORE_CHECK),
+ *     and bytes [0, out_size[i]) of slot i are its output, those delivered before an error included.
+ *   - Nothing outside [out_off[i], out_off[i] + out_cap[i]) is written.  Inside a slot, bytes past out_size[i] may be
+ *     written only when ret[i] != XZB_OK (later Blocks of a failed Stream may already have been decoded there).
+ *   - n = 0, zero-length items and unaligned offsets are valid.
+ * The return value is for errors of the whole call (device, memory). */
+int xzb_stream_buffer_decode_batch_device(xzb_ctx *ctx, uint32_t n, const uint8_t *d_in, const uint64_t *in_off,
+		const uint64_t *in_size, uint8_t *d_out, const uint64_t *out_off, const uint64_t *out_cap,
+		uint64_t *out_size, uint64_t *in_used, uint32_t *ret, uint32_t flags);
 
 /*
  * DECODE, device-resident Blocks: comp_off[i]/comp_size[i] locate Block i's LZMA2 payload

@@ -5,8 +5,10 @@ Jobs: 4096 x 128 KiB of `T` at -6 with CRC32 (one Stream per filesystem block), 
 CRC64.  For each job the probe reports MB/s of uncompressed data for
   * the batch: device-timed (CUDA events of the call, xzb_stats.ms_total) and end to end (host clock around the
     Python call, packing of the items and copies included);
-  * a loop of single calls (xzb_stream_buffer_encode / _decode) over the first `--loop` items only, end to end.
-Every batch item is checked against the single call on that subset, and the batch decode against the input.
+  * a loop of single calls (xzb_stream_buffer_encode / _decode) over the first `--loop` items only, end to end;
+  * device-resident decode (xzb_stream_buffer_decode_batch_device) of the Streams that the device encode batch left in
+    HBM, into slots in HBM: device-timed, and end to end (host clock around the call, which ends in a synchronise).
+Every batch item is checked against the single call on that subset, and both batch decodes against the input.
 The card's name and power limit are read in the same run.  Prints one JSON line; --out DIR also writes it there.
 
     python profiles/batch_probe.py [--loop 64] [--out DIR]
@@ -61,13 +63,42 @@ def run_job(ctx, name, count, size, preset, check, loop):
         r, out, _ = ctx.stream_buffer_decode(s, size)
         assert r == 0
     t_dec_loop = time.perf_counter() - t0
+    dd_dev_ms, t_dd = device_decode(ctx, whole, count, size, preset, check)
     mbs = lambda nbytes, sec: round(nbytes / sec / 1e6, 2)
     return {"job": name, "items": count, "item_bytes": size, "preset": preset, "check": check,
             "ratio": round(total / sum(len(s) for s in streams), 3),
             "encode_batch_MBps_device": mbs(total, enc_dev_ms / 1e3), "encode_batch_MBps_e2e": mbs(total, t_enc),
             "encode_loop_MBps_e2e": mbs(loop * size, t_enc_loop),
             "decode_batch_MBps_device": mbs(total, dec_dev_ms / 1e3), "decode_batch_MBps_e2e": mbs(total, t_dec),
-            "decode_loop_MBps_e2e": mbs(loop * size, t_dec_loop), "loop_items": loop}
+            "decode_loop_MBps_e2e": mbs(loop * size, t_dec_loop), "loop_items": loop,
+            "decode_device_batch_MBps_device": mbs(total, dd_dev_ms / 1e3), "decode_device_batch_MBps_e2e": mbs(total, t_dd)}
+
+
+def device_decode(ctx, whole, count, size, preset, check):
+    """(device ms, host seconds) of the device-resident decode of the job's Streams, made by the device encode batch."""
+    import xz_b200
+    cap = xz_b200.lib().xzb_stream_buffer_bound(size)
+    d_src, d_xz, d_back = ctx.device_alloc(len(whole)), ctx.device_alloc(cap * count), ctx.device_alloc(len(whole))
+    try:
+        ctx.h2d(d_src, whole, len(whole))
+        offs = [i * size for i in range(count)]
+        xz_offs = [i * cap for i in range(count)]
+        enc = ctx.stream_buffer_encode_batch_device(d_src, offs, [size] * count, xz_b200.lzma_lzma_preset(preset), check, d_xz, xz_offs,
+                                                    [cap] * count)
+        assert all(r == 0 for r, _ in enc)
+        sizes = [s for _, s in enc]
+        ctx.stream_buffer_decode_batch_device(d_xz, xz_offs[:8], sizes[:8], d_back, offs[:8], [size] * 8)  # warm-up
+        t0 = time.perf_counter()
+        dec = ctx.stream_buffer_decode_batch_device(d_xz, xz_offs, sizes, d_back, offs, [size] * count)
+        t = time.perf_counter() - t0
+        dev_ms = ctx.stats().ms_total
+        assert dec == [(0, size, s) for s in sizes]
+        back = bytearray(len(whole))
+        ctx.d2h(back, d_back, len(whole))
+        assert bytes(back) == whole, "device decode did not return the items"
+    finally:
+        ctx.device_free(d_src); ctx.device_free(d_xz); ctx.device_free(d_back)
+    return dev_ms, t
 
 
 def main():

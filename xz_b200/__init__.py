@@ -83,6 +83,7 @@ def lib():
         L.xzb_stream_buffer_encode_batch_device.argtypes = L.xzb_stream_buffer_encode_batch.argtypes
         L.xzb_stream_buffer_decode_batch.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, P64, P64, C.c_void_p, P64, P64, P64, P64, P32,
                                                      C.c_uint32]
+        L.xzb_stream_buffer_decode_batch_device.argtypes = L.xzb_stream_buffer_decode_batch.argtypes
         L.xzb_stream_decode.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64)]
         L.xzb_decode_blocks_device.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64), C.POINTER(C.c_uint64),
                                                C.POINTER(C.c_uint64), C.POINTER(C.c_uint32), C.c_uint32, C.c_uint32, C.c_void_p,
@@ -258,6 +259,21 @@ class Context:
             raise XzError(r, self._err())
         raw = C.string_at(out, len(out))
         return [(rets[i], raw[out_off[i]: out_off[i] + size[i]], used[i]) for i in range(n)]
+
+    def stream_buffer_decode_batch_device(self, d_in, in_off, in_size, d_out, out_off, out_cap, flags=0):
+        """The decode batch on device memory: d_in / d_out are addresses (or CUDA tensors; synchronise their stream
+        first), the offset and size lists stay on the host.  Returns [(ret, output size, input bytes used)]; item i's
+        output is at d_out + out_off[i]."""
+        n = len(in_off)
+        A = C.c_uint64 * max(n, 1)
+        size, used, rets = A(), A(), (C.c_uint32 * max(n, 1))()
+        ip, _k1 = _ptr(d_in)
+        op, _k2 = _ptr(d_out)
+        r = lib().xzb_stream_buffer_decode_batch_device(self._h, n, ip, A(*in_off), A(*in_size), op, A(*out_off), A(*out_cap), size,
+                                                        used, rets, flags)
+        if r != LZMA_OK:
+            raise XzError(r, self._err())
+        return [(rets[i], size[i], used[i]) for i in range(n)]
 
     # ---- lzma_stream_decoder + lzma_code(FINISH) on host buffers ----
     def stream_decode_into(self, src, n, dst, cap):

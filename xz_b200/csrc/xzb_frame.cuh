@@ -1,5 +1,5 @@
 // xzb_frame.cuh -- the .xz container: framing around the LZMA2 payload of one block, plus the
-// Stream Header / Index / Stream Footer, written (host/device) and read back (host only, at the end).
+// Stream Header / Index / Stream Footer, written and read back (host and device).
 // Reference: common/block_header_encoder.c, common/block_encoder.c:104-133,
 // common/block_buffer_encoder.c:27-162, common/vli_encoder.c, common/index_encoder.c:43-165,
 // common/stream_flags_encoder.c:29-85; the read side: common/vli_decoder.c,
@@ -209,19 +209,16 @@ XZB_HD uint64_t xzb_pack_stream(const uint32_t *crc32_table, uint8_t *dst, const
 	return xzb_oneshot_stream_size(block_size, unpadded, uncomp);
 }
 
-// ---- read side (host only), over untrusted input: every reader stays inside the `size` / `avail` bytes it is given ----
-static inline uint32_t xzb_check_field_size(uint32_t check)  // any of the 16 Check IDs, supported or not (check.c:62-86)
-{
-	static const uint8_t sizes[16] = { 0, 4, 4, 4, 8, 8, 8, 16, 16, 16, 32, 32, 32, 64, 64, 64 };
-	return check > 15 ? 0xFFFFFFFFu : sizes[check];
-}
+// ---- read side (host and device), over untrusted input: every reader stays inside the `size` / `avail` bytes it is given ----
+// any of the 16 Check IDs, supported or not (check.c:62-86): 0, then 4, 8, 16, 32, 64 bytes for three IDs each
+XZB_HD uint32_t xzb_check_field_size(uint32_t check) { return check > 15 ? 0xFFFFFFFFu : check == 0 ? 0 : 4u << ((check - 1) / 3); }
 
-static inline uint32_t xzb_rd32(const uint8_t *p) { return p[0] | ((uint32_t)p[1] << 8) | ((uint32_t)p[2] << 16) | ((uint32_t)p[3] << 24); }
+XZB_HD uint32_t xzb_rd32(const uint8_t *p) { return p[0] | ((uint32_t)p[1] << 8) | ((uint32_t)p[2] << 16) | ((uint32_t)p[3] << 24); }
 
 // lzma_vli_decode (single call), vli_decoder.c:16-86.  Whatever the result, *v has the bits read so far and *pos is past
 // the last byte read, so that a lax reader can still use what a strict one rejects.  LONG and NONMIN are invalid.
 enum { XZB_VLI_OK, XZB_VLI_SHORT /* input ran out */, XZB_VLI_LONG /* no last byte in nine */, XZB_VLI_NONMIN /* last byte 0x00 */ };
-static inline int xzb_vli_get(const uint8_t *in, uint64_t *pos, uint64_t size, uint64_t *v)
+XZB_HD int xzb_vli_get(const uint8_t *in, uint64_t *pos, uint64_t size, uint64_t *v)
 {
 	*v = 0;
 	for (uint32_t i = 0; i < 9; ++i) {
@@ -232,20 +229,19 @@ static inline int xzb_vli_get(const uint8_t *in, uint64_t *pos, uint64_t size, u
 	}
 	return XZB_VLI_LONG;
 }
-static inline int xzb_vli_verdict(int st) { return st == XZB_VLI_OK ? XZB_OK : st == XZB_VLI_SHORT ? XZB_BUF_ERROR : XZB_DATA_ERROR; }
+XZB_HD int xzb_vli_verdict(int st) { return st == XZB_VLI_OK ? XZB_OK : st == XZB_VLI_SHORT ? XZB_BUF_ERROR : XZB_DATA_ERROR; }
 
 // Stream Header / Footer, stream_flags_decoder.c:26-83, with the verdicts in the reference's order.  Comparing the
 // footer's Index size and Check ID with the Index and the Stream Header is the caller's.
-static inline int xzb_stream_header_decode(const uint32_t *crc32_table, const uint8_t in[12], uint32_t *check)
+XZB_HD int xzb_stream_header_decode(const uint32_t *crc32_table, const uint8_t in[12], uint32_t *check)
 {
-	static const uint8_t magic[6] = { 0xFD, 0x37, 0x7A, 0x58, 0x5A, 0x00 };
-	for (int i = 0; i < 6; ++i) if (in[i] != magic[i]) return XZB_FORMAT_ERROR;
+	if (in[0] != 0xFD || in[1] != 0x37 || in[2] != 0x7A || in[3] != 0x58 || in[4] != 0x5A || in[5] != 0x00) return XZB_FORMAT_ERROR;
 	if (xzb_crc32_bytes(crc32_table, in + 6, 2, 0) != xzb_rd32(in + 8)) return XZB_DATA_ERROR;
 	if (in[6] != 0x00 || (in[7] & 0xF0)) return XZB_OPTIONS_ERROR;
 	*check = in[7] & 0x0F;
 	return XZB_OK;
 }
-static inline int xzb_stream_footer_decode(const uint32_t *crc32_table, const uint8_t in[12], uint32_t *check, uint64_t *index_size)
+XZB_HD int xzb_stream_footer_decode(const uint32_t *crc32_table, const uint8_t in[12], uint32_t *check, uint64_t *index_size)
 {
 	if (in[10] != 'Y' || in[11] != 'Z' || xzb_crc32_bytes(crc32_table, in + 4, 6, 0) != xzb_rd32(in)) return XZB_DATA_ERROR;
 	if (in[8] != 0x00 || (in[9] & 0xF0)) return XZB_OPTIONS_ERROR;
@@ -259,7 +255,7 @@ static inline int xzb_stream_footer_decode(const uint32_t *crc32_table, const ui
 // absent one is 0, zero bytes long, OK.  No CRC32 or filter checks.  False when the header is not all in `avail`.
 struct XzbVliField { uint64_t v; uint32_t end; int st; };
 struct XzbBlockFraming { uint32_t hsize; uint8_t flags; XzbVliField comp, uncomp; };
-static inline bool xzb_block_framing(const uint8_t *h, uint64_t avail, XzbBlockFraming *f)
+XZB_HD bool xzb_block_framing(const uint8_t *h, uint64_t avail, XzbBlockFraming *f)
 {
 	f->hsize = ((uint32_t)h[0] + 1) * 4;
 	if (avail < f->hsize) return false;
@@ -280,7 +276,7 @@ struct XzbBlockHeader {
 	uint32_t n_pre;                // filters in front of LZMA2, in chain (= encoding) order
 	XzbPreFilter pre[3];
 };
-static inline int xzb_block_header_decode(const uint32_t *crc32_table, const uint8_t *h, uint64_t avail, XzbBlockHeader *hb)
+XZB_HD int xzb_block_header_decode(const uint32_t *crc32_table, const uint8_t *h, uint64_t avail, XzbBlockHeader *hb)
 {
 	XzbBlockFraming f;
 	if (!xzb_block_framing(h, avail, &f)) return XZB_BUF_ERROR;
@@ -336,11 +332,11 @@ struct XzbIndexRead {
 	uint64_t end;    // when listed: just past the CRC32 (the records rounded up to four bytes, + 4)
 	uint64_t stop;   // where a strict reader stops: just past the first fault, else = end
 };
-static inline int xzb_index_read(const uint32_t *crc32_table, const uint8_t *in, uint64_t size, const XzbIndexWant *want, XzbIndexRead *x)
+XZB_HD int xzb_index_read(const uint32_t *crc32_table, const uint8_t *in, uint64_t size, const XzbIndexWant *want, XzbIndexRead *x)
 {
 	uint64_t pos = 1, u = 0, w = 0;
 	int ret = XZB_OK, st;
-	auto fault = [&](int verdict) { if (ret == XZB_OK && verdict != XZB_OK) { ret = verdict; x->stop = pos; } };
+#define fault(verdict) do { const int v_ = (verdict); if (ret == XZB_OK && v_ != XZB_OK) { ret = v_; x->stop = pos; } } while (0)
 	fault(xzb_vli_verdict(st = xzb_vli_get(in, &pos, size, &x->count)));
 	if (want != nullptr && x->count != want->n) fault(XZB_DATA_ERROR);
 	for (uint64_t r = 0; st != XZB_VLI_SHORT && r < x->count; ++r) {
@@ -352,6 +348,7 @@ static inline int xzb_index_read(const uint32_t *crc32_table, const uint8_t *in,
 	x->end = ((pos + 3) & ~(uint64_t)3) + 4;
 	while (ret == XZB_OK && (pos & 3)) fault(pos >= size ? XZB_BUF_ERROR : in[pos++] != 0x00 ? XZB_DATA_ERROR : XZB_OK);
 	if (size - pos < 4) fault(XZB_BUF_ERROR);
+#undef fault
 	if (ret != XZB_OK) return ret;
 	uint32_t crc = 0xFFFFFFFFu;  // xzb_crc32_bytes for a 64-bit length
 	for (uint64_t i = 0; i < pos; ++i) crc = crc32_table[(crc ^ in[i]) & 0xFF] ^ (crc >> 8);

@@ -9,7 +9,8 @@
 //   xzb_k_parse_dp | xzb_k_parse_fast  1 CUDA block / .xz block : parser + range coder + LZMA2 chunker
 //   xzb_k_finalize    1 CUDA block / .xz block : header, padding, check | raw fallback
 //   xzb_k_pack_streams  1 CUDA block / .xz block : the finished Block to its place (+ Stream framing for one-shot items)
-// Decode: xzb_k_decode (1 CUDA block / .xz block) + xzb_k_crc over the output.
+// Decode: xzb_k_decode (1 CUDA block / .xz block) + xzb_k_crc over the output; the device-resident batch adds
+// xzb_k_dec_scan / xzb_k_dec_prep / xzb_k_dec_settle / xzb_k_dec_results, which read the container on the GPU.
 // There is deliberately no CPU path in this file.
 #include <cuda_runtime.h>
 #include <cub/cub.cuh>
@@ -28,6 +29,7 @@
 #include "xzb_dec_warp.cuh"
 #include "xzb_sha256.cuh"
 #include "xzb_frame.cuh"
+#include "xzb_dec_stream.cuh"
 #include "xzb_filters.cuh"
 #include "xzb_params.h"
 #include "xzb_parse_warp.cuh"
@@ -198,15 +200,18 @@ xzb_k_bt(const XzbMfBlock *__restrict__ blocks, XzbParams P, const uint32_t *__r
 // CRC of each block: slice 0 (short) starts from the real init value, the other slices from
 // zero; Z = "advance the register over L zero bytes" as a 64x64 GF(2) matrix (one column per
 // thread), then thread 0 folds the slices left to right.  Reflected CRC, check/crc64_fast.c
-// and crc32_fast.c compute the same polynomial division.
+// and crc32_fast.c compute the same polynomial division.  count (when given): the number of jobs, in device memory, for
+// a launch sized before it was known; CTAs past it return.
 struct XzbCrcJob { const uint8_t *data; uint32_t size; };
 
 __global__ void __launch_bounds__(1024)
-xzb_k_crc(const XzbCrcJob *__restrict__ jobs, const uint64_t *__restrict__ table, uint64_t init, uint64_t *__restrict__ out, uint32_t out_stride)
+xzb_k_crc(const XzbCrcJob *__restrict__ jobs, const uint64_t *__restrict__ table, uint64_t init, uint64_t *__restrict__ out, uint32_t out_stride,
+		const uint32_t *count)
 {
 	__shared__ uint64_t s_tab[256];
 	__shared__ uint64_t s_part[1024];
 	__shared__ uint64_t s_z[64];
+	if (count != nullptr && blockIdx.x >= *count) return;
 	const XzbCrcJob job = jobs[blockIdx.x];
 	const uint32_t T = blockDim.x;
 	const uint32_t t = threadIdx.x;
@@ -243,11 +248,11 @@ xzb_k_crc(const XzbCrcJob *__restrict__ jobs, const uint64_t *__restrict__ table
 }
 
 // SHA-256 of each block (LZMA_CHECK_SHA256): thread 0 of CTA b hashes block b; the chain is serial per
-// message, the wave's blocks give the parallelism.  out: 32 bytes per block.
+// message, the wave's blocks give the parallelism.  out: 32 bytes per block.  count: as for xzb_k_crc.
 __global__ void __launch_bounds__(32)
-xzb_k_sha256(const XzbCrcJob *__restrict__ jobs, uint8_t *__restrict__ out)
+xzb_k_sha256(const XzbCrcJob *__restrict__ jobs, uint8_t *__restrict__ out, const uint32_t *count)
 {
-	if (threadIdx.x != 0) return;
+	if (threadIdx.x != 0 || (count != nullptr && blockIdx.x >= *count)) return;
 	const XzbCrcJob job = jobs[blockIdx.x];
 	uint8_t digest[32];
 	xzb_sha256(job.data, job.size, digest);
@@ -516,7 +521,6 @@ struct XzbDecJob {
 	uint32_t out_limit;
 	uint32_t dict_size;
 };
-struct XzbDecResult { uint32_t ret, in_used, out_used, pad_; };
 
 // One warp per .xz block; the probability model lives in shared memory (28 KB, so several blocks
 // share an SM), every lane runs the (inherently serial) bit decoding uniformly, lane 0 stores
@@ -531,6 +535,125 @@ xzb_k_decode(const XzbDecJob *__restrict__ jobs, XzbDecResult *__restrict__ resu
 	uint32_t iu = 0, ou = 0;
 	const int ret = xzb_lzma2_decode(d, job.in, job.in_size, job.dict_size, job.out, job.out_limit, &iu, &ou, threadIdx.x, 32);
 	if (threadIdx.x == 0) { results[b].ret = (uint32_t)ret; results[b].in_used = iu; results[b].out_used = ou; }
+}
+
+// ---- device-resident Stream decode (xzb_stream_buffer_decode_batch_device) ----
+// Each round: xzb_k_dec_scan (the next run of every unfinished item, xzb_dec_scan) -> xzb_k_decode over the run's
+// Blocks -> xzb_k_dec_prep (filter and check job lists) -> xzb_k_filter per chain level -> xzb_k_crc / xzb_k_sha256
+// -> xzb_k_dec_settle (xzb_dec_settle, and xzb_dec_end at the Index).  The cursors stay in HBM between rounds.
+struct XzbDecItem {             // item i of a group: its Stream, its output slot, its Index record area
+	const uint8_t *in;
+	uint8_t *out;
+	xzb_index_record *recs;
+	uint64_t rec_cap;
+};
+struct XzbDecRound { uint32_t job0, nb, chk0, pad_; };   // the item's run in the round's job list; its first check job
+struct XzbDecCounters {
+	uint32_t njobs;             // jobs asked for (may exceed the round's capacity; the grants stop there)
+	uint32_t depth;             // longest Delta / BCJ chain in front of LZMA2 among the round's Blocks
+	uint32_t checks;            // check lists in use: 1 CRC32, 2 CRC64, 4 SHA-256
+	uint32_t live;              // items not finished after xzb_k_dec_settle
+	uint32_t nchk[3];           // jobs of the CRC32, CRC64 and SHA-256 lists
+	uint32_t pad_;
+	unsigned long long positions;  // bytes of the validated Blocks (kept over the rounds)
+};
+struct XzbDecOut { uint64_t out_size, in_used; uint32_t ret, pad_; };
+
+XZB_HD uint32_t xzb_dec_check_list(uint32_t check) { return check == 1 ? 0 : check == 4 ? 1 : 2; }
+
+// One thread per item.  The run is scanned twice: once to learn its length, which reserves that many job slots, and
+// again into the slots granted (a prefix of the run when the round's capacity runs out; the rest waits a round).
+__global__ void __launch_bounds__(128)
+xzb_k_dec_scan(XzbDecCursor *__restrict__ cur, const XzbDecItem *__restrict__ items, uint32_t n, const uint32_t *__restrict__ crc32_table,
+		uint32_t cap, XzbDecBlk *__restrict__ blks, XzbDecJob *__restrict__ jobs, XzbDecRound *__restrict__ round, XzbDecCounters *cnt)
+{
+	const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+	if (i >= n) return;
+	round[i].nb = 0;
+	if (cur[i].done) return;
+	const XzbDecItem it = items[i];
+	XzbDecCursor c = cur[i];
+	const uint32_t want = xzb_dec_scan(c, it.in, crc32_table, nullptr, cap, it.recs);
+	if (want == 0) { cur[i] = c; return; }   // finished by its header or at its Index
+	const uint32_t base = atomicAdd(&cnt->njobs, want);
+	if (base >= cap) return;
+	c = cur[i];
+	const uint32_t nb = xzb_dec_scan(c, it.in, crc32_table, blks + base, min(want, cap - base), it.recs);
+	uint32_t depth = 0;
+	for (uint32_t b = 0; b < nb; ++b) {
+		const XzbDecBlk &k = blks[base + b];
+		XzbDecJob j;
+		j.in = it.in + k.hdr_off + k.hb.hsize; j.in_size = k.in_avail;
+		j.out = it.out + k.out_off; j.out_limit = k.out_limit; j.dict_size = k.hb.dict_size;
+		jobs[base + b] = j;
+		depth = max(depth, k.hb.n_pre);
+	}
+	round[i] = XzbDecRound{ base, nb, 0, 0 };
+	if (depth) atomicMax(&cnt->depth, depth);
+	const uint32_t ck = xzb_dec_check_computed(c);
+	if (ck) atomicOr(&cnt->checks, 1u << xzb_dec_check_list(ck));
+	cur[i] = c;
+}
+
+// One thread per item of the round: the filter jobs of every chain level (in reverse chain order, size 0 where the
+// Block's chain is shorter) and the item's Blocks as one stretch of its check list.
+__global__ void __launch_bounds__(128)
+xzb_k_dec_prep(const XzbDecCursor *__restrict__ cur, XzbDecRound *__restrict__ round, uint32_t n, const XzbDecBlk *__restrict__ blks,
+		const XzbDecJob *__restrict__ jobs, const XzbDecResult *__restrict__ results, uint32_t cap, XzbFiltJob *__restrict__ filt,
+		XzbCrcJob *__restrict__ chk_jobs, XzbDecCounters *cnt)
+{
+	const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+	if (i >= n) return;
+	const XzbDecRound r = round[i];
+	if (r.nb == 0) return;
+	const uint32_t depth = cnt->depth;
+	for (uint32_t b = 0; b < r.nb; ++b) {
+		const uint32_t j = r.job0 + b;
+		const XzbBlockHeader &hb = blks[j].hb;
+		for (uint32_t lvl = 0; lvl < depth; ++lvl) {
+			XzbFiltJob f{ jobs[j].out, jobs[j].out, 0, 0, 0, 0 };
+			if (lvl < hb.n_pre) { const XzbPreFilter p = hb.pre[hb.n_pre - 1 - lvl]; f.size = results[j].out_used; f.id = p.id; f.arg = p.arg; }
+			filt[(size_t)lvl * cap + j] = f;
+		}
+	}
+	const uint32_t ck = xzb_dec_check_computed(cur[i]);
+	if (ck == 0) return;
+	const uint32_t list = xzb_dec_check_list(ck);
+	const uint32_t k0 = atomicAdd(&cnt->nchk[list], r.nb);
+	round[i].chk0 = k0;
+	for (uint32_t b = 0; b < r.nb; ++b) chk_jobs[(size_t)list * cap + k0 + b] = XzbCrcJob{ jobs[r.job0 + b].out, results[r.job0 + b].out_used };
+}
+
+// One thread per item: xzb_dec_settle over the item's run against the checks computed for it, counting the items
+// that still have Blocks to go.
+__global__ void __launch_bounds__(128)
+xzb_k_dec_settle(XzbDecCursor *__restrict__ cur, const XzbDecItem *__restrict__ items, const XzbDecRound *__restrict__ round, uint32_t n,
+		const uint32_t *__restrict__ crc32_table, const XzbDecBlk *__restrict__ blks, const XzbDecResult *__restrict__ results, uint32_t cap,
+		const uint64_t *__restrict__ crcv, const uint8_t *__restrict__ shav, XzbDecCounters *cnt)
+{
+	const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+	if (i >= n) return;
+	const XzbDecRound r = round[i];
+	if (r.nb == 0) { if (!cur[i].done) atomicAdd(&cnt->live, 1u); return; }
+	XzbDecCursor c = cur[i];
+	const XzbDecItem it = items[i];
+	const uint32_t list = xzb_dec_check_list(c.check);
+	const uint8_t *chk = list == 2 ? shav + 32 * (size_t)r.chk0 : (const uint8_t *)(crcv + (size_t)list * cap + r.chk0);
+	const uint64_t produced = xzb_dec_settle(c, it.in, crc32_table, blks + r.job0, results + r.job0, chk, list == 2 ? 32 : 8, it.recs, it.rec_cap);
+	if (produced) atomicAdd(&cnt->positions, (unsigned long long)produced);
+	if (!c.done) atomicAdd(&cnt->live, 1u);
+	cur[i] = c;
+}
+
+// The results with xzb_stream_buffer_decode()'s mapping: input that ended early is XZB_DATA_ERROR.
+__global__ void __launch_bounds__(128)
+xzb_k_dec_results(const XzbDecCursor *__restrict__ cur, uint32_t n, XzbDecOut *__restrict__ out)
+{
+	const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+	if (i >= n) return;
+	const XzbDecCursor c = cur[i];
+	const int code = c.ret == XZB_BUF_ERROR && c.buf_reason == 1 ? XZB_DATA_ERROR : c.ret;
+	out[i] = XzbDecOut{ c.out_size, c.in_used, (uint32_t)code, 0 };
 }
 
 // ------------------------------------------------------------------------------------
@@ -967,7 +1090,7 @@ static int encode_wave(xzb_ctx *ctx, const uint8_t *d_in, uint64_t in_bytes, con
 	auto launch_crc = [&]() {
 		if (check == 1 || check == 4) {
 			const bool c64 = check == 4;
-			xzb_k_crc<<<B, 1024, 0, st>>>(d_crcjobs, c64 ? ctx->d_crc64 : ctx->d_crc32w, c64 ? ~0ull : 0xFFFFFFFFull, d_crcv, 4);
+			xzb_k_crc<<<B, 1024, 0, st>>>(d_crcjobs, c64 ? ctx->d_crc64 : ctx->d_crc32w, c64 ? ~0ull : 0xFFFFFFFFull, d_crcv, 4, nullptr);
 			++launches;
 		}
 	};
@@ -996,7 +1119,7 @@ static int encode_wave(xzb_ctx *ctx, const uint8_t *d_in, uint64_t in_bytes, con
 		xzb_k_hc<<<2 * ntiles, 128, 0, st>>>(d_blocks, d_tiles, d_woff, P);
 		++launches;
 		CK(cudaEventRecord(ctx->ev[2], st));
-		if (check == 10) { xzb_k_sha256<<<B, 32, 0, st>>>(d_crcjobs, (uint8_t *)d_crcv); ++launches; }
+		if (check == 10) { xzb_k_sha256<<<B, 32, 0, st>>>(d_crcjobs, (uint8_t *)d_crcv, nullptr); ++launches; }
 	} else {
 		// Beside the parser the search keeps off the parser's SMs (see xzb_k_bt): the launch is
 		// oversubscribed by the CTAs that will retire there, `live` CTAs do the work.
@@ -1021,7 +1144,7 @@ static int encode_wave(xzb_ctx *ctx, const uint8_t *d_in, uint64_t in_bytes, con
 		CK(cudaEventRecord(ctx->ev_mf[1], st_mf));
 		if (!overlap) CK(cudaEventRecord(ctx->ev[2], st));
 		// SHA-256 needs only the input: behind the search on its stream, i.e. beside the parser when overlapping
-		if (check == 10) { xzb_k_sha256<<<B, 32, 0, st_mf>>>(d_crcjobs, (uint8_t *)d_crcv); ++launches; CK(cudaEventRecord(ctx->ev_mf[2], st_mf)); }
+		if (check == 10) { xzb_k_sha256<<<B, 32, 0, st_mf>>>(d_crcjobs, (uint8_t *)d_crcv, nullptr); ++launches; CK(cudaEventRecord(ctx->ev_mf[2], st_mf)); }
 	}
 	launch_crc();
 	CK(cudaEventRecord(ctx->ev[3], st));
@@ -1462,11 +1585,11 @@ static int decode_batch(xzb_ctx *ctx, const std::vector<XzbDecJob> &jobs, const 
 		CK(cudaMemcpyAsync(sm + off_crcjobs, cj.data(), sizeof(XzbCrcJob) * nc, cudaMemcpyHostToDevice, st));
 		std::vector<uint8_t> got(32 * (size_t)nc);
 		if (c == 10) {
-			xzb_k_sha256<<<nc, 32, 0, st>>>((const XzbCrcJob *)(sm + off_crcjobs), sm + off_crcv);
+			xzb_k_sha256<<<nc, 32, 0, st>>>((const XzbCrcJob *)(sm + off_crcjobs), sm + off_crcv, nullptr);
 			CK(cudaMemcpyAsync(got.data(), sm + off_crcv, 32 * (size_t)nc, cudaMemcpyDeviceToHost, st));
 		} else {
 			const bool c64 = c == 4;
-			xzb_k_crc<<<nc, 1024, 0, st>>>((const XzbCrcJob *)(sm + off_crcjobs), c64 ? ctx->d_crc64 : ctx->d_crc32w, c64 ? ~0ull : 0xFFFFFFFFull, (uint64_t *)(sm + off_crcv), 1);
+			xzb_k_crc<<<nc, 1024, 0, st>>>((const XzbCrcJob *)(sm + off_crcjobs), c64 ? ctx->d_crc64 : ctx->d_crc32w, c64 ? ~0ull : 0xFFFFFFFFull, (uint64_t *)(sm + off_crcv), 1, nullptr);
 			CK(cudaMemcpyAsync(got.data(), sm + off_crcv, 8 * (size_t)nc, cudaMemcpyDeviceToHost, st));
 		}
 		ctx->stats.gpu_launches += 1;
@@ -1576,51 +1699,18 @@ extern "C" int xzb_stream_decode_flags(xzb_ctx *ctx, const uint8_t *in, uint64_t
 	return xzb_stream_decode_prior(ctx, in, in_size, out, out_cap, out_size, in_used, flags, nullptr, 0);
 }
 
-// One Stream in flight in decode_streams(): the caller's view, and the decoder's cursor over it.
+// One Stream in flight in decode_streams(): the caller's view, and the decoder's cursor over it (xzb_dec_stream.cuh).
 struct XzbDecStream {
 	const uint8_t *in; uint64_t in_size;     // host
 	uint8_t *out; uint64_t out_cap;          // host
 	uint32_t flags;
 	const xzb_index_record *prior; uint64_t n_prior;  // see xzb_stream_decode_prior
-	// results
-	int ret = XZB_OK;
-	int buf_reason = 1;                      // why XZB_BUF_ERROR: 1 = the input ended early, 2 = the output is too small
-	uint64_t in_used = 0, out_size = 0;
-	// cursor
-	bool done = false, at_index = false;
-	uint32_t check = 0, csize = 0;
-	bool verify = true;
-	uint64_t d_in = 0, d_out = 0;            // its input / output in ctx->dec_in / ctx->dec_out
-	uint64_t ip = 12, op = 0;
+	XzbDecCursor c;
 	std::vector<xzb_index_record> recs;
-	// the Blocks of the current round
-	std::vector<XzbBlockHeader> batch;
-	std::vector<uint64_t> hdr_offs, out_offs;
-	std::vector<bool> truncated, out_exact;
-	uint64_t bip = 0;
-	int pending = XZB_OK;                    // error discovered while scanning ahead: reported after the round
+	std::vector<XzbDecBlk> blks;             // the Blocks of the current round
+	uint64_t d_in = 0, d_out = 0;            // its input / output in ctx->dec_in / ctx->dec_out
 	size_t job0 = 0;
 };
-
-// Index + Stream Footer behind the last Block (common/index_hash.c:175-341, stream_decoder.c:266-332), then the
-// Stream's results.
-static void decode_stream_end(xzb_ctx *ctx, XzbDecStream &s)
-{
-	if (s.ret == XZB_OK) {
-		const XzbIndexWant want{ s.recs.data(), s.recs.size() };
-		XzbIndexRead x;
-		s.ret = xzb_index_read(ctx->h_tab.crc32, s.in + s.ip, s.in_size - s.ip, &want, &x);
-		s.ip += x.stop;
-		uint32_t fcheck = 0; uint64_t fisize = 0;
-		if (s.ret == XZB_OK && s.in_size - s.ip < 12) s.ret = XZB_BUF_ERROR;
-		if (s.ret == XZB_OK) s.ret = xzb_stream_footer_decode(ctx->h_tab.crc32, s.in + s.ip, &fcheck, &fisize);
-		if (s.ret == XZB_OK && (fisize != x.end || fcheck != s.check)) s.ret = XZB_DATA_ERROR;
-		if (s.ret == XZB_OK) s.ip += 12;
-	}
-	s.in_used = s.ip;
-	s.out_size = s.op;
-	s.done = true;
-}
 
 // Decodes the Streams S side by side.  Their inputs go to HBM in one copy of the span they cover; each round scans the
 // next run of sized Blocks of every unfinished Stream (an unsized Block gets a round of its own), decodes all of them
@@ -1629,17 +1719,13 @@ static void decode_stream_end(xzb_ctx *ctx, XzbDecStream &s)
 static int decode_streams(xzb_ctx *ctx, std::vector<XzbDecStream> &S)
 {
 	cudaStream_t st = ctx->stream;
+	const uint32_t *crc32 = ctx->h_tab.crc32;
 	const uint8_t *lo = nullptr, *hi = nullptr;
 	uint64_t out_total = 0;
 	for (XzbDecStream &s : S) {
+		xzb_dec_init(s.c, s.in_size, s.out_cap, s.flags, s.n_prior);
 		s.recs.assign(s.prior, s.prior + s.n_prior);
-		if (s.in_size < 12) { s.ret = XZB_BUF_ERROR; s.done = true; continue; }
-		const int hr = xzb_stream_header_decode(ctx->h_tab.crc32, s.in, &s.check);
-		if (hr != XZB_OK) { s.ret = hr; s.done = true; continue; }
-		s.csize = xzb_check_field_size(s.check);
-		// Checks other than CRC32 / CRC64 / SHA-256 are reserved IDs: like the reference
-		// (block_decoder.c:178-190 compares only when lzma_check_is_supported()) they are skipped.
-		s.verify = !(s.flags & XZB_DEC_IGNORE_CHECK);  // LZMA_IGNORE_CHECK, stream_decoder.c:188-190
+		if (!xzb_dec_header(s.c, s.in, crc32)) continue;
 		if (lo == nullptr || s.in < lo) lo = s.in;
 		if (hi == nullptr || s.in + s.in_size > hi) hi = s.in + s.in_size;
 		s.d_out = out_total;
@@ -1663,45 +1749,23 @@ static int decode_streams(xzb_ctx *ctx, std::vector<XzbDecStream> &S)
 		std::vector<XzbDecStream *> round;
 		bool any_chain = false;
 		for (XzbDecStream &s : S) {
-			if (s.done || jobs.size() >= 4096) continue;
-			// gather a run of blocks whose headers carry both sizes (stream_decoder_mt.c:862-931)
-			s.batch.clear(); s.hdr_offs.clear(); s.out_offs.clear();
-			s.pending = XZB_OK;
-			s.bip = s.ip;
-			uint64_t bop = s.op;
-			for (;;) {
-				if (s.bip >= s.in_size) { s.pending = XZB_BUF_ERROR; break; }
-				if (s.in[s.bip] == 0x00) { s.at_index = true; break; }
-				XzbBlockHeader hb;
-				const int r = xzb_block_header_decode(ctx->h_tab.crc32, s.in + s.bip, s.in_size - s.bip, &hb);
-				if (r != XZB_OK) { s.pending = r; break; }
-				const bool sized = hb.comp != UINT64_MAX && hb.uncomp != UINT64_MAX;
-				if (!sized && !s.batch.empty()) break;  // decode what we have first
-				s.batch.push_back(hb); s.hdr_offs.push_back(s.bip); s.out_offs.push_back(bop);
-				if (!sized) break;  // direct mode: one block at a time
-				const uint64_t padded = (hb.comp + 3) & ~3ull;
-				if (s.in_size - (s.bip + hb.hsize) < padded + s.csize || s.out_cap - bop < hb.uncomp) break;  // let the per-block logic report it
-				s.bip += hb.hsize + padded + s.csize; bop += hb.uncomp;
-				if (jobs.size() + s.batch.size() >= 4096) break;
-			}
-			if (s.batch.empty()) { s.ret = s.pending; decode_stream_end(ctx, s); continue; }
+			if (s.c.done || jobs.size() >= 4096) continue;
+			// the run's length first, as xzb_k_dec_scan learns it, then the run into an array of that size
+			XzbDecCursor probe = s.c;
+			const uint32_t nb = xzb_dec_scan(probe, s.in, crc32, nullptr, (uint32_t)(4096 - jobs.size()), s.recs.data());
+			if (nb == 0) { s.c = probe; continue; }
+			s.blks.resize(nb);
+			xzb_dec_scan(s.c, s.in, crc32, s.blks.data(), nb, s.recs.data());
 			s.job0 = jobs.size();
-			s.truncated.assign(s.batch.size(), true); s.out_exact.assign(s.batch.size(), false);
-			for (size_t b = 0; b < s.batch.size(); ++b) {
-				const XzbBlockHeader &hb = s.batch[b];
-				const uint64_t dpos = s.hdr_offs[b] + hb.hsize;
-				uint64_t in_avail = s.in_size - dpos;
-				if (hb.comp != UINT64_MAX && hb.comp <= in_avail) { in_avail = hb.comp; s.truncated[b] = false; }
-				uint64_t out_limit = s.out_cap - s.out_offs[b];
-				if (hb.uncomp != UINT64_MAX && hb.uncomp <= out_limit) { out_limit = hb.uncomp; s.out_exact[b] = true; }
-				if (in_avail > 0xFFFFFFF0ull || out_limit > 0xFFFFFFF0ull) { in_avail = std::min<uint64_t>(in_avail, 0xFFFFFFF0ull); out_limit = std::min<uint64_t>(out_limit, 0xFFFFFFF0ull); }
+			for (uint32_t b = 0; b < nb; ++b) {
+				const XzbDecBlk &k = s.blks[b];
 				XzbDecJob j;
-				j.in = d_in + s.d_in + dpos; j.in_size = (uint32_t)in_avail;
-				j.out = d_out + s.d_out + s.out_offs[b]; j.out_limit = (uint32_t)out_limit; j.dict_size = hb.dict_size;
+				j.in = d_in + s.d_in + k.hdr_off + k.hb.hsize; j.in_size = k.in_avail;
+				j.out = d_out + s.d_out + k.out_off; j.out_limit = k.out_limit; j.dict_size = k.hb.dict_size;
 				jobs.push_back(j);
-				checks.push_back(s.verify ? s.check : 0);
-				hdrs.push_back(hb);
-				any_chain = any_chain || hb.n_pre != 0;
+				checks.push_back(xzb_dec_check_computed(s.c));
+				hdrs.push_back(k.hb);
+				any_chain = any_chain || k.hb.n_pre != 0;
 			}
 			round.push_back(&s);
 		}
@@ -1711,49 +1775,17 @@ static int decode_streams(xzb_ctx *ctx, std::vector<XzbDecStream> &S)
 		if (r != XZB_OK) return r;
 		for (XzbDecStream *sp : round) {
 			XzbDecStream &s = *sp;
-			// per-block validation in stream order: common/block_decoder.c:64-200.  Like the reference
-			// (lz_decoder.c:128-160 copies what was decoded before it looks at the return code), the bytes a
-			// failing Block produced before the error are still delivered.
-			for (size_t b = 0; b < s.batch.size() && s.ret == XZB_OK; ++b) {
-				const XzbBlockHeader &hb = s.batch[b];
-				const size_t j = s.job0 + b;
-				const XzbDecResult &res = results[j];
-				const uint64_t op_fail = s.out_offs[b] + res.out_used;
-				int ret = XZB_OK;
-				if (res.ret == XZB_NEED_INPUT) ret = s.truncated[b] ? XZB_BUF_ERROR : XZB_DATA_ERROR;
-				else if (res.ret == XZB_NEED_OUTPUT) { ret = s.out_exact[b] ? XZB_DATA_ERROR : XZB_BUF_ERROR; s.buf_reason = 2; }
-				else if (res.ret != XZB_OK) ret = (int)res.ret;
-				else if ((hb.comp != UINT64_MAX && res.in_used != hb.comp) || (hb.uncomp != UINT64_MAX && res.out_used != hb.uncomp)) ret = XZB_DATA_ERROR;
-				uint64_t p = s.hdr_offs[b] + hb.hsize + res.in_used;
-				uint64_t c = res.in_used;
-				while (ret == XZB_OK && (c & 3)) {
-					if (p >= s.in_size) ret = XZB_BUF_ERROR;
-					else if (s.in[p++] != 0x00) ret = XZB_DATA_ERROR;
-					++c;
-				}
-				if (ret == XZB_OK && s.in_size - p < s.csize) ret = XZB_BUF_ERROR;
-				if (ret == XZB_OK && s.verify) {
-					const uint8_t *f = s.in + p;
-					if (s.check == 1) { if ((uint32_t)crcs[j] != xzb_rd32(f)) ret = XZB_DATA_ERROR; }
-					else if (s.check == 4) { if (crcs[j] != ((uint64_t)xzb_rd32(f) | ((uint64_t)xzb_rd32(f + 4) << 32))) ret = XZB_DATA_ERROR; }
-					else if (s.check == 10) { if (memcmp(shas.data() + 32 * j, f, 32) != 0) ret = XZB_DATA_ERROR; }
-				}
-				s.ret = ret;
-				if (ret != XZB_OK) { s.op = op_fail; break; }
-				p += s.csize;
-				xzb_index_record rec; rec.unpadded_size = hb.hsize + res.in_used + s.csize; rec.uncompressed_size = res.out_used;
-				s.recs.push_back(rec);
-				s.ip = p; s.op = s.out_offs[b] + res.out_used;
-				ctx->stats.n_positions += res.out_used;
-			}
-			if (s.ret == XZB_OK && s.pending != XZB_OK && s.ip == s.bip) s.ret = s.pending;
-			if (s.ret != XZB_OK || s.at_index) decode_stream_end(ctx, s);
+			const bool sha = s.c.check == 10;
+			const uint8_t *chk = sha ? shas.data() + 32 * s.job0 : (const uint8_t *)(crcs.data() + s.job0);
+			s.recs.resize(s.c.n_recs + s.c.nb);  // a round appends at most one record per Block
+			ctx->stats.n_positions += xzb_dec_settle(s.c, s.in, crc32, s.blks.data(), results.data() + s.job0, chk, sha ? 32 : 8,
+					s.recs.data(), s.recs.size());
 		}
 	}
 	// bytes of successfully validated blocks are delivered even when a later block fails
 	CK(cudaEventRecord(ctx->ev[10], st));
 	for (const XzbDecStream &s : S)
-		if (s.out_size > 0) CK(cudaMemcpyAsync(s.out, d_out + s.d_out, s.out_size, cudaMemcpyDeviceToHost, st));
+		if (s.c.out_size > 0) CK(cudaMemcpyAsync(s.out, d_out + s.d_out, s.c.out_size, cudaMemcpyDeviceToHost, st));
 	CK(cudaEventRecord(ctx->ev[11], st));
 	CK(cudaEventRecord(ctx->ev[7], st));
 	CK(cudaStreamSynchronize(st));
@@ -1783,10 +1815,10 @@ extern "C" int xzb_stream_decode_prior(xzb_ctx *ctx, const uint8_t *in, uint64_t
 	S[0].prior = prior; S[0].n_prior = n_prior;
 	const int r = decode_streams(ctx, S);
 	if (r != XZB_OK) return r;
-	*in_used = S[0].in_used;
-	*out_size = S[0].out_size;
-	ctx->dec_buf_reason = S[0].buf_reason;
-	return S[0].ret;
+	*in_used = S[0].c.in_used;
+	*out_size = S[0].c.out_size;
+	ctx->dec_buf_reason = S[0].c.buf_reason;
+	return S[0].c.ret;
 }
 
 // n independent Streams with xzb_stream_buffer_decode()'s result mapping per item.  Items go to the device in groups
@@ -1818,9 +1850,9 @@ extern "C" int xzb_stream_buffer_decode_batch(xzb_ctx *ctx, uint32_t n, const ui
 		const int r = decode_streams(ctx, S);
 		if (r != XZB_OK) return r;
 		for (uint32_t k = 0; k < S.size(); ++k) {
-			int code = S[k].ret;
-			if (code == XZB_BUF_ERROR && S[k].buf_reason == 1) code = XZB_DATA_ERROR;   // as xzb_stream_buffer_decode()
-			ret[i0 + k] = (uint32_t)code; out_size[i0 + k] = S[k].out_size; in_used[i0 + k] = S[k].in_used;
+			int code = S[k].c.ret;
+			if (code == XZB_BUF_ERROR && S[k].c.buf_reason == 1) code = XZB_DATA_ERROR;   // as xzb_stream_buffer_decode()
+			ret[i0 + k] = (uint32_t)code; out_size[i0 + k] = S[k].c.out_size; in_used[i0 + k] = S[k].c.in_used;
 		}
 		sum.ms_total += ctx->stats.ms_total; sum.ms_h2d += ctx->stats.ms_h2d; sum.ms_d2h += ctx->stats.ms_d2h;
 		sum.ms_decode += ctx->stats.ms_decode; sum.ms_other += ctx->stats.ms_other; sum.gpu_launches += ctx->stats.gpu_launches;
@@ -1829,6 +1861,143 @@ extern "C" int xzb_stream_buffer_decode_batch(xzb_ctx *ctx, uint32_t n, const ui
 		i0 = i;
 	}
 	ctx->stats = sum;
+	return XZB_OK;
+}
+
+// ------------------------------------------------------------------------------------
+// Decode, device-resident batch
+// ------------------------------------------------------------------------------------
+static const uint32_t XZB_DEC_ROUND_JOBS = 65536;  // Blocks decoded per round at most (the job area's capacity)
+
+static size_t dec_align(size_t v) { return (v + 255) & ~(size_t)255; }
+
+// HBM of one round's job area of `cap` jobs.
+static size_t dec_job_area(uint32_t cap)
+{
+	return dec_align(sizeof(XzbDecCounters)) + dec_align(sizeof(XzbDecBlk) * cap) + dec_align(sizeof(XzbDecJob) * cap)
+		+ dec_align(sizeof(XzbDecResult) * cap) + dec_align(sizeof(XzbFiltJob) * 3 * (size_t)cap) + dec_align(sizeof(XzbCrcJob) * 3 * (size_t)cap)
+		+ dec_align(8 * 2 * (size_t)cap) + dec_align(32 * (size_t)cap);
+}
+static const uint64_t XZB_DEC_ITEM_BYTES = sizeof(XzbDecCursor) + sizeof(XzbDecItem) + sizeof(XzbDecRound) + sizeof(XzbDecOut);
+
+// One group of items, all rounds.  Fills out_size / in_used / ret of items [i0, i0 + ng).
+static int decode_group_device(xzb_ctx *ctx, uint32_t ng, const uint8_t *d_in, const uint64_t *in_off, const uint64_t *in_size,
+		uint8_t *d_out, const uint64_t *out_off, const uint64_t *out_cap, uint64_t *out_size, uint64_t *in_used, uint32_t *ret, uint32_t flags)
+{
+	cudaStream_t st = ctx->stream;
+	uint64_t recs_total = 0;
+	for (uint32_t i = 0; i < ng; ++i) recs_total += xzb_dec_rec_bound(in_size[i]);
+	const uint32_t cap = (uint32_t)std::min<uint64_t>(XZB_DEC_ROUND_JOBS, recs_total);
+	// layout: counters, job area, then the per-item arrays and record areas
+	size_t o = 0;
+	auto take = [&](size_t bytes) { const size_t at = o; o += dec_align(bytes); return at; };
+	const size_t o_cnt = take(sizeof(XzbDecCounters)), o_blk = take(sizeof(XzbDecBlk) * cap), o_job = take(sizeof(XzbDecJob) * cap);
+	const size_t o_res = take(sizeof(XzbDecResult) * cap), o_filt = take(sizeof(XzbFiltJob) * 3 * (size_t)cap);
+	const size_t o_cj = take(sizeof(XzbCrcJob) * 3 * (size_t)cap), o_crcv = take(8 * 2 * (size_t)cap), o_shav = take(32 * (size_t)cap);
+	const size_t o_cur = take(sizeof(XzbDecCursor) * ng), o_item = take(sizeof(XzbDecItem) * ng), o_round = take(sizeof(XzbDecRound) * ng);
+	const size_t o_out = take(sizeof(XzbDecOut) * ng), o_recs = take(sizeof(xzb_index_record) * recs_total);
+	EN(ctx->decs, o);
+	uint8_t *base = (uint8_t *)ctx->decs.p;
+	XzbDecCounters *cnt = (XzbDecCounters *)(base + o_cnt);
+	XzbDecBlk *blks = (XzbDecBlk *)(base + o_blk);
+	XzbDecJob *jobs = (XzbDecJob *)(base + o_job);
+	XzbDecResult *res = (XzbDecResult *)(base + o_res);
+	XzbFiltJob *filt = (XzbFiltJob *)(base + o_filt);
+	XzbCrcJob *cj = (XzbCrcJob *)(base + o_cj);
+	uint64_t *crcv = (uint64_t *)(base + o_crcv);
+	uint8_t *shav = base + o_shav;
+	XzbDecCursor *cur = (XzbDecCursor *)(base + o_cur);
+	XzbDecItem *items = (XzbDecItem *)(base + o_item);
+	XzbDecRound *round = (XzbDecRound *)(base + o_round);
+	XzbDecOut *outs = (XzbDecOut *)(base + o_out);
+	xzb_index_record *recs = (xzb_index_record *)(base + o_recs);
+	// the cursors and where each item's bytes are: per-item metadata, no item data
+	std::vector<XzbDecCursor> hc(ng);
+	std::vector<XzbDecItem> hi(ng);
+	uint64_t r0 = 0;
+	for (uint32_t i = 0; i < ng; ++i) {
+		xzb_dec_init(hc[i], in_size[i], out_cap[i], flags, 0);
+		const uint64_t rc = xzb_dec_rec_bound(in_size[i]);
+		hi[i] = XzbDecItem{ d_in + in_off[i], d_out + out_off[i], recs + r0, rc };
+		r0 += rc;
+	}
+	CK(cudaMemcpyAsync(cur, hc.data(), sizeof(XzbDecCursor) * ng, cudaMemcpyHostToDevice, st));
+	CK(cudaMemcpyAsync(items, hi.data(), sizeof(XzbDecItem) * ng, cudaMemcpyHostToDevice, st));
+	CK(cudaMemsetAsync(cnt, 0, sizeof(XzbDecCounters), st));
+	const uint32_t grid_items = (ng + 127) / 128;
+	XzbDecCounters h;
+	for (;;) {
+		CK(cudaMemsetAsync(cnt, 0, offsetof(XzbDecCounters, positions), st));
+		xzb_k_dec_scan<<<grid_items, 128, 0, st>>>(cur, items, ng, ctx->d_crc32, cap, blks, jobs, round, cnt);
+		CK(cudaMemcpyAsync(&h, cnt, sizeof(h), cudaMemcpyDeviceToHost, st));
+		CK(cudaStreamSynchronize(st));
+		ctx->stats.gpu_launches += 1;
+		const uint32_t nj = std::min(h.njobs, cap);
+		if (nj == 0) break;   // every item finished at its header or its Index
+		CK(cudaEventRecord(ctx->ev[0], st));
+		xzb_k_decode<<<nj, 32, sizeof(XzbDec), st>>>(jobs, res);
+		CK(cudaEventRecord(ctx->ev[1], st));
+		xzb_k_dec_prep<<<grid_items, 128, 0, st>>>(cur, round, ng, blks, jobs, res, cap, filt, cj, cnt);
+		ctx->stats.gpu_launches += 2;
+		// Delta / BCJ behind LZMA2 (common/filter_decoder.c:44-139), undone in reverse chain order before the checks
+		for (uint32_t lvl = 0; lvl < h.depth; ++lvl) { xzb_k_filter<<<nj, 256, 0, st>>>(filt + (size_t)lvl * cap, 0); ctx->stats.gpu_launches += 1; }
+		for (uint32_t list = 0; list < 3; ++list) {
+			if (!(h.checks & (1u << list))) continue;
+			if (list == 2) xzb_k_sha256<<<nj, 32, 0, st>>>(cj + 2 * (size_t)cap, shav, &cnt->nchk[2]);
+			else xzb_k_crc<<<nj, 1024, 0, st>>>(cj + (size_t)list * cap, list ? ctx->d_crc64 : ctx->d_crc32w, list ? ~0ull : 0xFFFFFFFFull,
+					crcv + (size_t)list * cap, 1, &cnt->nchk[list]);
+			ctx->stats.gpu_launches += 1;
+		}
+		xzb_k_dec_settle<<<grid_items, 128, 0, st>>>(cur, items, round, ng, ctx->d_crc32, blks, res, cap, crcv, shav, cnt);
+		CK(cudaEventRecord(ctx->ev[2], st));
+		CK(cudaMemcpyAsync(&h, cnt, sizeof(h), cudaMemcpyDeviceToHost, st));
+		CK(cudaStreamSynchronize(st));
+		CK(cudaGetLastError());
+		ctx->stats.gpu_launches += 1;
+		ctx->stats.ms_decode += ev_ms(ctx->ev[0], ctx->ev[1]);
+		ctx->stats.n_blocks += nj;
+		if (h.live == 0) break;
+	}
+	xzb_k_dec_results<<<grid_items, 128, 0, st>>>(cur, ng, outs);
+	ctx->stats.gpu_launches += 1;
+	std::vector<XzbDecOut> ho(ng);
+	CK(cudaMemcpyAsync(ho.data(), outs, sizeof(XzbDecOut) * ng, cudaMemcpyDeviceToHost, st));
+	CK(cudaMemcpyAsync(&h, cnt, sizeof(h), cudaMemcpyDeviceToHost, st));
+	CK(cudaStreamSynchronize(st));
+	CK(cudaGetLastError());
+	ctx->stats.n_positions += h.positions;
+	for (uint32_t i = 0; i < ng; ++i) { ret[i] = ho[i].ret; out_size[i] = ho[i].out_size; in_used[i] = ho[i].in_used; }
+	return XZB_OK;
+}
+
+// xzb_stream_buffer_decode_batch with the Streams and the output slots in device memory: the container is read on the
+// GPU (xzb_dec_stream.cuh) and every Block decodes straight into its item's slot.  Items go in groups whose cursors
+// and Index record areas fit the memory budget beside one round's job area.
+extern "C" int xzb_stream_buffer_decode_batch_device(xzb_ctx *ctx, uint32_t n, const uint8_t *d_in, const uint64_t *in_off,
+		const uint64_t *in_size, uint8_t *d_out, const uint64_t *out_off, const uint64_t *out_cap, uint64_t *out_size, uint64_t *in_used,
+		uint32_t *ret, uint32_t flags)
+{
+	cudaSetDevice(ctx->device);
+	memset(&ctx->stats, 0, sizeof(ctx->stats));
+	ctx->err[0] = 0;
+	if (n == 0) return XZB_OK;
+	cudaStream_t st = ctx->stream;
+	CK(cudaEventRecord(ctx->ev[6], st));
+	size_t free_b = 0, total_b = 0;
+	cudaMemGetInfo(&free_b, &total_b);
+	const uint64_t avail = (uint64_t)((free_b + ctx->decs.cap) * 0.85), jobs = dec_job_area(XZB_DEC_ROUND_JOBS);
+	std::vector<uint32_t> start;
+	xzb_plan_dec_groups(in_size, n, XZB_DEC_ITEM_BYTES, avail > jobs ? avail - jobs : 0, &start);
+	for (size_t g = 0; g + 1 < start.size(); ++g) {
+		const uint32_t i0 = start[g], ng = start[g + 1] - i0;
+		const int r = decode_group_device(ctx, ng, d_in, in_off + i0, in_size + i0, d_out, out_off + i0, out_cap + i0, out_size + i0,
+				in_used + i0, ret + i0, flags);
+		if (r != XZB_OK) return r;
+	}
+	CK(cudaEventRecord(ctx->ev[7], st));
+	CK(cudaStreamSynchronize(st));
+	ctx->stats.ms_total = ev_ms(ctx->ev[6], ctx->ev[7]);
+	ctx->stats.ms_other = std::max(0.0, ctx->stats.ms_total - ctx->stats.ms_decode);
 	return XZB_OK;
 }
 

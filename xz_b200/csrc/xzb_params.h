@@ -131,6 +131,22 @@ static inline uint64_t xzb_wave_offsets(const uint32_t *n, uint32_t B, uint32_t 
 	return pos;
 }
 
+// Groups of the device-resident Stream decoder (xzb_stream_buffer_decode_batch_device): items in call order, item i
+// costing per_item + 16 * (in_size[i] / 16 + 1) bytes of HBM (its cursor and its Index record area, xzb_dec_rec_bound);
+// a group takes items while their sum stays within budget, and always at least one.  group_start: the first item of
+// each group, plus n.
+static inline void xzb_plan_dec_groups(const uint64_t *in_size, uint32_t n, uint64_t per_item, uint64_t budget, std::vector<uint32_t> *group_start)
+{
+	group_start->clear();
+	uint64_t used = 0;
+	for (uint32_t i = 0; i < n; ++i) {
+		const uint64_t c = per_item + 16 * (in_size[i] / 16 + 1);
+		if (i == 0 || used + c > budget) { group_start->push_back(i); used = 0; }
+		used += c;
+	}
+	group_start->push_back(n);
+}
+
 struct XzbHostTables { uint32_t crc32[256]; uint64_t crc64[256]; uint8_t prices[128]; };
 
 static inline void xzb_make_tables(XzbHostTables *t)
