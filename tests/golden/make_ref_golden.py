@@ -4,7 +4,7 @@
 
 The reference's answers on the tests' seeded inputs (filters, encoders, decoder verdicts, the <lzma.h>
 struct layout, `xz -6 -T1` Streams, the LZMA2 option sweep of test_gpu_option_sweep.py and its Streams with rewritten
-dictionary sizes), stored as the first 48 bits of SHA-256.
+dictionary sizes, the decoder's verdicts on the Streams of tests/lzma2_gen.py), stored as the first 48 bits of SHA-256.
 """
 import ctypes as C
 import json
@@ -22,6 +22,7 @@ import test_filters_cpu as F
 import test_gpu_filters as G
 import test_gpu_option_sweep as S
 import test_oracle as O
+import lzma2_gen
 
 sys.path.insert(0, os.path.dirname(TESTS))
 REF = __import__("__graft_entry__").reference_tree()   # the reference source tree (for its public header)
@@ -75,6 +76,23 @@ def dict_header():
     return out
 
 
+def lzma2_gen_section():
+    """The single-threaded and threaded decoders' [ret, out_size, output] on each generated Stream, and the
+    single-threaded decoder's on the same Stream without the Block Header's size fields.  A valid case's output must be
+    the generator's plaintext: a generator bug is not recorded as the reference's answer."""
+    out = {}
+    for c in lzma2_gen.cases():
+        unsized = X.drop_block_sizes(c.xz)
+        res = [X.ref_decode(c.xz, c.declared), X.ref_decode(c.xz, c.declared, mt=True), X.ref_decode(unsized, c.declared)]
+        for r, back in res:
+            if c.verdict == 0:
+                assert r == 0 and back == c.expected, (c.name, r, len(back))
+            else:
+                assert r == c.verdict, (c.name, r)
+        out[c.name] = {"stream": sha(c.xz), "decode": [[r, len(back), sha(back)] for r, back in res]}
+    return out
+
+
 def main():
     assert X.have_ref(), "oracle/_ref is not built"
     assert REF and os.path.isdir(REF), "the reference source tree is not there (XZ_REFERENCE)"
@@ -105,6 +123,7 @@ def main():
         g["mf_encode"][O.mf_key(o)] = sha(X.ref_encode(buf, 300000, 0, 1 << 20, opts=o))
     g["opt_sweep"] = opt_sweep()
     g["dict_header"] = dict_header()
+    g["lzma2_gen"] = lzma2_gen_section()
     with tempfile.TemporaryDirectory() as d:
         src = os.path.join(d, "l.c")
         open(src, "w").write(API.LAYOUT_PROG.replace("HEADER", "<lzma.h>"))

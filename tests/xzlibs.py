@@ -90,7 +90,12 @@ def drop_block_sizes(xz):
             _, q = _read_vli(xz, q)
         if flags & 0x80:
             _, q = _read_vli(xz, q)
-        filt = xz[q:pos + hs - 4].rstrip(b"\0")
+        f0 = q
+        for _ in range((flags & 3) + 1):   # Filter Flags: ID, Size of Properties, Properties (a property may be 0x00)
+            _, q = _read_vli(xz, q)
+            psize, q = _read_vli(xz, q)
+            q += psize
+        filt = xz[f0:q]
         body = bytes([flags & 0x3F]) + filt
         body += b"\0" * (-(len(body) + 5) % 4)
         hdr = bytes([(len(body) + 5) // 4 - 1]) + body
