@@ -57,6 +57,7 @@ typedef struct {
 	uint64_t n_symbols;    /* LZMA symbols emitted */
 	uint64_t n_chunks_lzma, n_chunks_raw;
 	uint64_t n_raw_with_read_ahead; /* D12 probe: raw chunk taken with read_ahead != 0 */
+	uint64_t n_raw_ahead_then_lzma; /* of those, the ones the next chunk of the same Block codes as LZMA */
 } xzo_counters;
 
 /* lzma_block_buffer_bound64(), src/liblzma/common/block_buffer_encoder.c:56-71 */

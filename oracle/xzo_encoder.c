@@ -1236,6 +1236,7 @@ static int lzma2_encode_block(enc_t *e, mf_t *mf, uint8_t *out, size_t out_cap, 
 {
 	size_t out_pos = *out_pos_ptr;
 	int need_properties = 1, need_state_reset = 0, need_dictionary_reset = 1;
+	int raw_with_read_ahead = 0; /* the last chunk was raw and swallowed read_ahead bytes */
 	uint8_t *buf = malloc(LZMA2_HEADER_MAX + LZMA2_CHUNK_MAX);
 	if (buf == NULL) return XZO_MEM_ERROR;
 	int ret = XZO_OK;
@@ -1259,6 +1260,7 @@ static int lzma2_encode_block(enc_t *e, mf_t *mf, uint8_t *out, size_t out_cap, 
 		if (compressed_size >= uncompressed_size) {
 			/* raw chunk :202-214, header :107-131, copy mf_read lz_encoder.h:302-318 */
 			if (e->ctr) { e->ctr->n_chunks_raw++; if (mf->read_ahead) e->ctr->n_raw_with_read_ahead++; }
+			raw_with_read_ahead = mf->read_ahead != 0;
 			uncompressed_size += mf->read_ahead;
 			mf->read_ahead = 0;
 			if (out_pos + 3 + uncompressed_size > out_cap) { ret = XZO_BUF_ERROR; break; }
@@ -1272,7 +1274,8 @@ static int lzma2_encode_block(enc_t *e, mf_t *mf, uint8_t *out, size_t out_cap, 
 			continue;
 		}
 		/* lzma2_header_lzma :53-104 */
-		if (e->ctr) e->ctr->n_chunks_lzma++;
+		if (e->ctr) { e->ctr->n_chunks_lzma++; e->ctr->n_raw_ahead_then_lzma += raw_with_read_ahead; }
+		raw_with_read_ahead = 0;
 		size_t pos;
 		if (need_properties) {
 			pos = 0;

@@ -4,7 +4,8 @@
 
 The reference's answers on the tests' seeded inputs (filters, encoders, decoder verdicts, the <lzma.h>
 struct layout, `xz -6 -T1` Streams, the LZMA2 option sweep of test_gpu_option_sweep.py and its Streams with rewritten
-dictionary sizes, the decoder's verdicts on the Streams of tests/lzma2_gen.py), stored as the first 48 bits of SHA-256.
+dictionary sizes, the decoder's verdicts on the Streams of tests/lzma2_gen.py, the Streams of the chunk-mix cases of
+tests/chunk_mix.py), stored as the first 48 bits of SHA-256.
 """
 import ctypes as C
 import json
@@ -23,6 +24,7 @@ import test_gpu_filters as G
 import test_gpu_option_sweep as S
 import test_oracle as O
 import lzma2_gen
+import chunk_mix
 
 sys.path.insert(0, os.path.dirname(TESTS))
 REF = __import__("__graft_entry__").reference_tree()   # the reference source tree (for its public header)
@@ -93,6 +95,22 @@ def lzma2_gen_section():
     return out
 
 
+def chunk_mix_section():
+    """lzma_stream_encoder_mt with each chunk-mix case's options ([LZMA chunks, uncompressed chunks] read from its
+    Blocks), and lzma_easy_buffer_encode of each one-shot item.  The oracle must write the same Stream: a difference is
+    an oracle bug, not an answer to record."""
+    out = {}
+    for c in chunk_mix.cases():
+        xz = X.ref_encode(c.data, len(c.data), 0, c.block_size, c.check, opts=c.opts)
+        assert X.oracle_encode(c.data, len(c.data), 0, c.block_size, c.check, opts=c.opts) == xz, c.name
+        out[chunk_mix.key(c)] = {"stream": sha(xz), "chunks": list(chunk_mix.chunk_counts(xz))}
+    for name, p, data in chunk_mix.oneshot_items():
+        xz = X.ref_buffer_encode(data, len(data), p)
+        assert X.oracle_buffer_encode(data, len(data), p) == xz, name
+        out[name] = {"stream": sha(xz)}
+    return out
+
+
 def main():
     assert X.have_ref(), "oracle/_ref is not built"
     assert REF and os.path.isdir(REF), "the reference source tree is not there (XZ_REFERENCE)"
@@ -124,6 +142,7 @@ def main():
     g["opt_sweep"] = opt_sweep()
     g["dict_header"] = dict_header()
     g["lzma2_gen"] = lzma2_gen_section()
+    g["chunk_mix"] = chunk_mix_section()
     with tempfile.TemporaryDirectory() as d:
         src = os.path.join(d, "l.c")
         open(src, "w").write(API.LAYOUT_PROG.replace("HEADER", "<lzma.h>"))

@@ -14,7 +14,8 @@ class LzmaOptions(C.Structure):
 
 class Counters(C.Structure):
     _fields_ = [(n, C.c_uint64) for n in ("n_pos", "n_nodes", "n_cmp_bytes", "n_pairs", "n_symbols",
-                                          "n_chunks_lzma", "n_chunks_raw", "n_raw_with_read_ahead")]
+                                          "n_chunks_lzma", "n_chunks_raw", "n_raw_with_read_ahead",
+                                          "n_raw_ahead_then_lzma")]
 
 
 _cache = {}
