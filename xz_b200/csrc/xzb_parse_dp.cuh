@@ -56,6 +56,12 @@ __device__ __forceinline__ uint4 dp_lds128(const volatile void *p)
 	asm volatile("ld.volatile.shared.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"((uint32_t)__cvta_generic_to_shared(const_cast<const void *>(p))) : "memory");
 	return v;
 }
+__device__ __forceinline__ uint2 dp_lds64(const volatile void *p)
+{
+	uint2 v;
+	asm volatile("ld.volatile.shared.v2.u32 {%0, %1}, [%2];" : "=r"(v.x), "=r"(v.y) : "r"((uint32_t)__cvta_generic_to_shared(const_cast<const void *>(p))) : "memory");
+	return v;
+}
 __device__ __forceinline__ void dp_sts128(volatile void *p, const uint4 v)
 {
 	asm volatile("st.volatile.shared.v4.u32 [%0], {%1, %2, %3, %4};" :: "r"((uint32_t)__cvta_generic_to_shared(const_cast<void *>(p))), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
@@ -792,20 +798,26 @@ __device__ inline void xzb_dp_worker_main(DS &S, DpEnc &H, const uint32_t w)
 				}
 			}
 			// =============== wait for the node itself ===============
+			const uint32_t k = c & rmask;
+			// Between here and the near-wave push nothing writes slots c + 2 and c + 3 of the own ring: this worker's earlier
+			// nodes are done, and the gather warp clears a slot only when it reads it, which waits for this node's wave 1.
+			// So the prices they hold now are the ones the push compares with, read off the path that follows the flag.
+			const uint32_t near_old = lane < 2 ? rg[(c + 2 + lane) & rmask].x : 0u;
 			DP_T(w0);
 			__syncwarp();
+			// The node record is loaded with every poll, after the flag: loads are performed in order, so when the flag says
+			// the node is final, the record loaded after it is the final one -- one shared-memory round trip less after the flag.
+			uint2 ni; uint4 rr;
 			for (uint32_t it = 0;; ++it) {
 				const uint32_t f = __shfl_sync(WFULL, S.fin_node, 0);
+				ni = dp_lds64(&S.n_info[k]); rr = dp_lds128(&S.n_reps[k]);
 				if ((f >> 16) == (want >> 16) && (f & 0xFFFF) >= c) break;
 				if ((it & 31) == 31 && __shfl_sync(WFULL, (uint32_t)(S.seg_stop != DP_NONE || S.seg_epoch != my_epoch || S.m_exit), 0)) { gone = true; break; }
 			}
 			if (gone) break;
 			DP_T(w1);
 			DP_ACQUIRE();
-			const uint32_t k = c & rmask;
-			const uint2 ni = S.n_info[k];
 			const uint32_t price = ni.x, st = ni.y & 0xFF, mb = ni.y >> 8;
-			const uint4 rr = S.n_reps[k];
 			const uint32_t hr[4] = { rr.x, rr.y, rr.z, rr.w };
 			const uint32_t baf = xzb_min(H.size - p, XZB_OPTS - 1 - c);   // buf_avail_full
 			const uint32_t nice_len = H.nice_len, pos_mask = H.pos_mask;
@@ -841,15 +853,17 @@ __device__ inline void xzb_dp_worker_main(DS &S, DpEnc &H, const uint32_t w)
 						const bool eqL = lane == 0 ? (mg0 & 3) == 0 : (mg0 & 7) == 0;
 						const bool vr = lane < 2 && eqL, vmn = lane < 2 && !eqL && L2 <= new_len;
 						const uint32_t lb = xzb_max((mg0 & 3) == 0 ? 2u : 0u, new_len >= 2 ? new_len : 0u);
-						if (lane == 0 && lb) atomicMax(&S.len_end_sh, c + lb);
 						uint32_t prn = 0, men = 0, bkn = 0;
 						const uint32_t nmb = __shfl_sync(WFULL, cvw, L2 & 7);   // rep0's bytes 0..7 sit in lanes 0..7
 						if (vr) { prn = price + b1.x + H.len_price(1, L2, ps); men = DP_META(L2, 0u, 0u, L2 < buf_avail ? nmb : (uint32_t)bb0[L2]); }
 						if (vmn) { const uint2 e2 = PL[L2 - 2]; prn = price + b0.y + (e2.x & 0xFFFF); men = DP_META(L2, 0u, 0u, e2.x >> 16); bkn = e2.y + XZB_REPS; }
-						H.push(rg, vr || vmn, c + L2, prn, bkn, men, 0);
+						if ((vr || vmn) && prn < near_old) rg[(c + L2) & rmask] = make_uint4(prn, bkn, men, 0u);   // H.push against near_old
 						__syncwarp();
 						near_done = true;
 						if (!lr_near) { DP_RELEASE(); if (lane == 0) S.ph[k] = (want << 2) | 1u; }
+						// len_end only has to grow before this node's last phase flag (the chain warp waits for every node to be
+						// complete before it ends the segment on len_end), so the atomic comes after the flag the gather waits for
+						if (lane == 0 && lb) atomicMax(&S.len_end_sh, c + lb);
 						{ DP_T(wn); if (lane == 0 && w == 0) { DP_ACC(29, w1, wn); DP_CNT(30); } }
 					}
 				}
