@@ -368,7 +368,7 @@ xzb_k_parse_dp(const XzbEncJob *__restrict__ jobs, const XzbMfBlock *__restrict_
 	if (threadIdx.x <= DP_WMAX) S.idle[threadIdx.x] = 0;
 	if (threadIdx.x < 32) { S.part_tag[threadIdx.x] = 0; S.res_c[threadIdx.x] = make_uint4(0u, 0u, 0u, 0u); }
 #ifdef XZB_DP_PROF
-	if (threadIdx.x < 32) S.prof[threadIdx.x] = 0;
+	if (threadIdx.x < 40) S.prof[threadIdx.x] = 0;
 #endif
 	for (uint32_t i = threadIdx.x; i < DP_NR; i += blockDim.x) S.ph[i] = 0;
 	__syncthreads();
@@ -417,6 +417,8 @@ xzb_k_parse_dp(const XzbEncJob *__restrict__ jobs, const XzbMfBlock *__restrict_
 			const double ns = (double)S.prof[15] + 1e-9, ng = (double)S.prof[19] + 1e-9;
 			printf("DPPROF symbols %llu: optimum_normal %.0f encode_symbol %.0f cyc/symbol | segments %llu: helper1 %.0f idle_wait %.0f backward %.0f cyc/segment\n",
 				S.prof[15], S.prof[13] / ns, S.prof[14] / ns, S.prof[19], S.prof[16] / ng, S.prof[17] / ng, S.prof[18] / ng);
+			printf("DPPROF coder ring full: %llu waits, %.0f Mcycles (%.0f cyc/segment) | seg_stop -> next segment's first fin_node: %.0f cyc x %llu (%.1f%% of the chain)\n",
+				S.prof[32], S.prof[31] / 1e6, S.prof[31] / ng, S.prof[33] / ((double)S.prof[34] + 1e-9), S.prof[34], 100.0 * (double)S.prof[33] / cyc);
 		}
 #endif
 	}

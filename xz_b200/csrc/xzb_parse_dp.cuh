@@ -137,7 +137,7 @@ struct DS {  // dynamic shared memory of xzb_k_parse_dp
 	volatile uint32_t rcq_flushes, rcq_out_pos;   // chunks finished, compressed size of the last one
 	volatile uint32_t part_tag[32];          // tagn(t) + 1
 #ifdef XZB_DP_PROF
-	unsigned long long prof[32];
+	unsigned long long prof[40];
 #endif
 };
 
@@ -146,6 +146,9 @@ struct DpEnc : WarpEncT<DS> {
 	uint32_t epoch;                           // chain warp: current segment
 	uint32_t sym_cur, sym_end;                // symbol stack [sym_cur, sym_end) left over from the last backward()
 	uint32_t *trace; uint32_t trace_cap, trace_n;
+#ifdef XZB_DP_PROF
+	long long t_stop = 0;                     // chain warp: clock64() when the last segment was stopped
+#endif
 
 	__device__ DpEnc(DS &s, uint32_t l) : WarpEncT<DS>(s, l) {}
 
@@ -492,6 +495,9 @@ struct DpEnc : WarpEncT<DS> {
 				DP_RELEASE();
 				*(volatile uint32_t *)&S.fin_node = tagn(epoch, cur);   // the owner of node cur may push now (n_c1 follows with nil_node)
 			}
+#ifdef XZB_DP_PROF
+			if (cur == 1 && t_stop != 0) { DP_T(f1); if (lane == 0) { DP_ACC(33, t_stop, f1); DP_CNT(34); } }   // seg_stop -> next first fin_node
+#endif
 			// first look at the gather warp's record for slot cur + 1 (usually there already; the loads overlap the pricing below)
 			const uint32_t wantp = tagn(epoch, cur + 1) + 1;
 			const volatile uint32_t *tp = &S.part_tag[(cur + 1) & 31];
@@ -533,6 +539,9 @@ struct DpEnc : WarpEncT<DS> {
 		__syncwarp();
 		if (lane == 0) { S.o_back[cur] = Wn.y; S.o_meta[cur] = Wn.z; S.o_back2[cur] = Wn.w; __threadfence_block(); S.seg_stop = cur; }
 		DP_T(i0);
+#ifdef XZB_DP_PROF
+		t_stop = i0;
+#endif
 		for (;;) {
 			const bool ok = lane > W || S.idle[lane] == epoch;
 			if (__all_sync(WFULL, ok)) break;
@@ -601,7 +610,15 @@ struct DpEnc : WarpEncT<DS> {
 			if (read_pos - read_ahead >= limit || rc_pending_reaches(XZB_LZMA2_CHUNK_MAX - XZB_LOOP_INPUT_MAX)) break;
 			if (read_pos >= size) { if (read_ahead == 0) break; }
 			if (mf_stalled) break;
-			while (rq_head - S.rcq_tail > DP_RCQ - 128u) { }   // ring space for one symbol (the coder warp is far faster than the DP)
+#ifdef XZB_DP_PROF
+			if (rq_head - S.rcq_tail > DP_RCQ - 128u) {
+				DP_T(q0);
+				while (rq_head - S.rcq_tail > DP_RCQ - 128u) { }
+				DP_T(q1);
+				if (lane == 0) { DP_ACC(31, q0, q1); DP_CNT(32); }
+			}
+#endif
+			while (rq_head - S.rcq_tail > DP_RCQ - 128u) { }   // ring space for one symbol
 			uint32_t len, back;
 			DP_T(e0);
 			optimum_normal(&back, &len, uncomp_size);

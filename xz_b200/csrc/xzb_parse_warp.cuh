@@ -358,28 +358,6 @@ struct WarpEncT {
 		rc_low = (rc_low & 0x00FFFFFF) << 8;
 	}
 
-	// one coded bit: p = probability before adaptation, 0xFFFF = direct bit (range_encoder.h:196-234)
-	__device__ __forceinline__ void rc_step(uint32_t p, uint32_t bit)
-	{
-		if (rc_range < (1u << 24)) { rc_shift_low(); rc_range <<= 8; }
-		if (p == 0xFFFF) {
-			rc_range >>= 1;
-			if (bit) rc_low += rc_range;
-		} else {
-			const uint32_t bound = (rc_range >> 11) * p;
-			if (bit) { rc_low += bound; rc_range -= bound; } else rc_range = bound;
-		}
-	}
-
-	// the same for a bit that is known to be probability-coded (no direct-bit test on the chain)
-	__device__ __forceinline__ void rc_step_prob(uint32_t p, uint32_t bit)
-	{
-		if (rc_range < (1u << 24)) { rc_shift_low(); rc_range <<= 8; }
-		const uint32_t bound = (rc_range >> 11) * p;
-		rc_low += bit ? bound : 0u;
-		rc_range = bit ? rc_range - bound : bound;
-	}
-
 	__device__ void rc_flush()  // rc_flush + RC_FLUSH handling, range_encoder.h:127-132, 198-203, 236-249
 	{
 		if constexpr (SM::RCQ != 0) {   // marker record; the coder warp flushes, then reports the chunk's size
@@ -848,27 +826,24 @@ __device__ inline void xzb_w_coder_main(SM &S, ENC &H)
 		if (fresh) { H.rc_out = S.rcq_out; H.rc_out_pos = 0; fresh = false; }
 		const uint32_t n = xzb_min(head - tail, 32u);
 		const uint32_t w = lane < n ? (uint32_t)S.rcq[(tail + lane) & (SM::RCQ - 1)] : 0u;
-		for (uint32_t i = 0; i < n; ++i) {
-			const uint32_t wi = __shfl_sync(WFULL, w, i);
-			if (wi & 0x8000u) {
-				if (H.rc_range < (1u << 24)) { H.rc_shift_low(); H.rc_range <<= 8; }
-				for (int k = 0; k < 5; ++k) H.rc_shift_low();
-				const uint32_t sz = H.rc_out_pos;
-				H.rc_low = 0; H.rc_cache_size = 1; H.rc_range = 0xFFFFFFFFu; H.rc_cache = 0; H.rc_out_pos = 0;
-				++flushes;
-				fresh = true;   // anything after a flush marker belongs to the next chunk; the coding warp waits for us first
-				__syncwarp();
-				if (lane == 0) {
-					S.rcq_out_pos = sz;
-					S.rcq_T = 1;
-					S.rcq_tail = tail + i + 1;
-					__threadfence_block();
-					S.rcq_flushes = flushes;
-				}
-			} else if (wi & 0x2000u) {
-				H.rc_step(0xFFFF, (wi >> 12) & 1);
-			} else {
-				H.rc_step_prob(wi & 0xFFF, (wi >> 12) & 1);
+		// A flush marker is the last record of a batch: the coding warp waits for the flush before it queues more.
+		const bool flush = (__shfl_sync(WFULL, w, n - 1) & 0x8000u) != 0;
+		// The batch goes through the coding warp's two-pass form; S.rc_bits is free in kernels with a coder warp.
+		S.rc_bits[lane] = (uint16_t)w;
+		__syncwarp();
+		H.rc_run32(0, flush ? n - 1 : n);
+		if (flush) {
+			H.rc_flush_local();
+			const uint32_t sz = H.rc_out_pos;
+			H.rc_out_pos = 0;
+			++flushes;
+			fresh = true;
+			if (lane == 0) {
+				S.rcq_out_pos = sz;
+				S.rcq_T = 1;
+				S.rcq_tail = tail + n;
+				__threadfence_block();
+				S.rcq_flushes = flushes;
 			}
 		}
 		tail += n;
