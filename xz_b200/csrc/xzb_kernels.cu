@@ -368,7 +368,7 @@ xzb_k_parse_dp(const XzbEncJob *__restrict__ jobs, const XzbMfBlock *__restrict_
 	if (threadIdx.x <= DP_WMAX) S.idle[threadIdx.x] = 0;
 	if (threadIdx.x < 32) { S.part_tag[threadIdx.x] = 0; S.res_c[threadIdx.x] = make_uint4(0u, 0u, 0u, 0u); }
 #ifdef XZB_DP_PROF
-	if (threadIdx.x < 40) S.prof[threadIdx.x] = 0;
+	if (threadIdx.x < 44) S.prof[threadIdx.x] = 0;
 #endif
 	for (uint32_t i = threadIdx.x; i < DP_NR; i += blockDim.x) S.ph[i] = 0;
 	__syncthreads();
@@ -415,8 +415,11 @@ xzb_k_parse_dp(const XzbEncJob *__restrict__ jobs, const XzbMfBlock *__restrict_
 				(double)S.prof[7] / ((double)S.prof[4] + 1e-9), (double)S.prof[29] / ((double)S.prof[30] + 1e-9), S.prof[30]);
 			printf("DPPROF gather: slots that had to wait for node t-2: %llu, t-3: %llu, t-4: %llu, t-5..8: %llu, older: %llu\n", S.prof[24], S.prof[25], S.prof[26], S.prof[27], S.prof[28]);
 			const double ns = (double)S.prof[15] + 1e-9, ng = (double)S.prof[19] + 1e-9;
-			printf("DPPROF symbols %llu: optimum_normal %.0f encode_symbol %.0f cyc/symbol | segments %llu: helper1 %.0f idle_wait %.0f backward %.0f cyc/segment\n",
-				S.prof[15], S.prof[13] / ns, S.prof[14] / ns, S.prof[19], S.prof[16] / ng, S.prof[17] / ng, S.prof[18] / ng);
+			printf("DPPROF symbols %llu: optimum_normal %.0f cyc/symbol, encode_symbol %.0f cyc x %llu, chunk-loop tests %.0f cyc/iteration | segments %llu: helper1 %.0f idle_wait %.0f backward %.0f cyc/segment\n",
+				S.prof[15], S.prof[13] / ns, S.prof[14] / ((double)S.prof[43] + 1e-9), S.prof[43], S.prof[42] / ((double)S.prof[36] + S.prof[43] + 1e-9), S.prof[19], S.prof[16] / ng, S.prof[17] / ng, S.prof[18] / ng);
+			const double nb = (double)S.prof[36] + 1e-9;
+			printf("DPPROF batches %llu: %.0f cyc, %.0f records, %.0f cyc waiting for ring space per batch; cut by a chunk limit %llu, then %llu symbols coded one by one; length-price refreshes inside %llu\n",
+				S.prof[36], S.prof[35] / nb, S.prof[37] / nb, S.prof[38] / nb, S.prof[39], S.prof[40], S.prof[41]);
 			printf("DPPROF coder ring full: %llu waits, %.0f Mcycles (%.0f cyc/segment) | seg_stop -> next segment's first fin_node: %.0f cyc x %llu (%.1f%% of the chain)\n",
 				S.prof[32], S.prof[31] / 1e6, S.prof[31] / ng, S.prof[33] / ((double)S.prof[34] + 1e-9), S.prof[34], 100.0 * (double)S.prof[33] / cyc);
 		}

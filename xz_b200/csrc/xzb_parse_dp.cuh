@@ -93,7 +93,7 @@ __device__ __forceinline__ void dp_sts128(volatile void *p, const uint4 v)
 //   z = buf[p] | buf[p-1] << 8, w = get_literal_price(..., match_mode = false, ...)
 typedef uint4 DpPrep;
 
-#define DP_RCQ 2048u                  // coded-bit ring to the coder warp (16-bit records)
+#define DP_RCQ 4096u                  // coded-bit ring to the coder warp (16-bit records); 4096: the coder warp keeps up with a batch (DESIGN.md section 8)
 struct DS {  // dynamic shared memory of xzb_k_parse_dp
 	static constexpr uint32_t RCQ = DP_RCQ;
 	static constexpr bool FAST = false;
@@ -137,7 +137,7 @@ struct DS {  // dynamic shared memory of xzb_k_parse_dp
 	volatile uint32_t rcq_flushes, rcq_out_pos;   // chunks finished, compressed size of the last one
 	volatile uint32_t part_tag[32];          // tagn(t) + 1
 #ifdef XZB_DP_PROF
-	unsigned long long prof[40];
+	unsigned long long prof[44];
 #endif
 };
 
@@ -588,6 +588,191 @@ struct DpEnc : WarpEncT<DS> {
 		pk = L | (lt2 << 9) | (mbt << 18);
 	}
 
+	__device__ __forceinline__ uint32_t sym_nbits(uint32_t back, uint32_t len, uint32_t ps) const
+	{
+		if (back == XZB_BACK_LITERAL) return 9;
+		const bool m = back >= XZB_REPS;
+		const uint32_t pre_n = m ? 2u : (back <= 1 ? 4u : 5u);
+		if (!m && len == 1) return pre_n;   // short rep
+		return LenDist(pre_n, m ? 0u : 1u, ps, len, m ? back - XZB_REPS : 0xFFFFFFFFu).n;
+	}
+
+	// ---- the run backward() just stacked, coded as one batch ----
+	// Codes the symbols from sym_cur - 1 (the one optimum_normal returned) on, with exactly encode_symbol's records and
+	// side effects, up to the first symbol before which one of encode_chunk's limit tests might hold: the uncompressed
+	// one is exact from the lengths; the compressed one takes the bound of rc_pending_reaches, read once, plus the
+	// records of the batch's earlier symbols (each record the coder warp takes meanwhile lowers the queue by one and
+	// raises its count by at most one).  The symbols from there on are left on the stack for the exact per-symbol loop.
+	//   32 symbols at a time, lane j = symbol j: lengths and record counts by warp scans, state and reps by a uniform
+	//   loop, the length-price counters per (coder, pos_state) group; each lane writes its symbol's records to a staging
+	//   area.  Then the records go out 32 at a time in coding order: equal probability indices of a window hand the value
+	//   on in lane order, and a window stops at the first record of a symbol whose length prices are refreshed
+	//   (length_count: the refresh sees every earlier symbol's adaptations and none of its own, DESIGN.md F2).
+	__device__ void encode_batch(uint32_t limit)
+	{
+		const uint32_t s0 = sym_cur - 1, n = sym_end - s0;
+		uint32_t cb0 = 0;
+		if (lane == 0) { const uint32_t tail = S.rcq_tail; asm volatile("" ::: "memory"); cb0 = S.rcq_T + (rq_head - tail) + 4; }
+		cb0 = __shfl_sync(WFULL, cb0, 0);
+		const uint32_t p0 = read_pos - read_ahead, lt = (1u << lane) - 1;
+		uint32_t *const len_ctr = &S.len_counters[0][0];   // [which * XZB_POS_STATES_MAX + pos_state]
+		// the records of 32 symbols (at most 48 each) are staged behind the symbol stack, in the workers' idle rings
+		static_assert((DP_POOL - XZB_OPTS / 2) * sizeof(uint4) >= 32 * 48 * sizeof(uint16_t), "batch staging");
+		uint16_t *const stg = reinterpret_cast<uint16_t *>(&S.ring_pool[XZB_OPTS / 2]);
+		uint32_t done = 0, off = 0, nrec = 0;   // symbols, bytes and records of the batch so far
+		bool cut = false;
+		while (done < n && !cut) {
+			const bool in = done + lane < n;
+			const uint2 sy = in ? sym_stack()[s0 + done + lane] : make_uint2(0u, 0u);
+			const uint32_t back = sy.x, len = sy.y;
+			const uint32_t pos = uncomp_size + off;   // + the lengths before this lane's symbol
+			uint32_t lx = len;
+#pragma unroll
+			for (uint32_t d = 1; d < 32; d <<= 1) { const uint32_t o = __shfl_up_sync(WFULL, lx, d); if (lane >= d) lx += o; }
+			lx -= len;
+			const uint32_t ps = (pos + lx) & pos_mask;
+			const uint32_t nb = in ? sym_nbits(back, len, ps) : 0u;
+			uint32_t bx = nb;
+#pragma unroll
+			for (uint32_t d = 1; d < 32; d <<= 1) { const uint32_t o = __shfl_up_sync(WFULL, bx, d); if (lane >= d) bx += o; }
+			bx -= nb;
+			const bool stop = in && done + lane != 0 && (p0 + off + lx >= limit || cb0 + nrec + bx >= XZB_LZMA2_CHUNK_MAX - XZB_LOOP_INPUT_MAX);
+			const uint32_t sm = __ballot_sync(WFULL, stop);
+			const uint32_t nw = sm ? (uint32_t)__ffs((int)sm) - 1 : xzb_min(n - done, 32u);
+			cut = sm != 0;
+			if (nw == 0) break;
+			const bool v = lane < nw;
+			// state and reps before each symbol (encode_symbol's updates); they end before the first symbol not coded
+			uint32_t st = 0, r0 = 0;
+			for (uint32_t u = 0; u < nw; ++u) {
+				const uint32_t b = __shfl_sync(WFULL, back, u), l = __shfl_sync(WFULL, len, u);
+				if (lane == u) { st = state; r0 = rep0; }
+				const bool hi = state >= XZB_LIT_STATES;
+				if (b == XZB_BACK_LITERAL) {
+					state = hi ? (state <= 9 ? state - 3 : state - 6) : (state <= 3 ? 0 : state - 3);
+				} else if (b >= XZB_REPS) {
+					state = hi ? 10 : 7;
+					rep3 = rep2; rep2 = rep1; rep1 = rep0; rep0 = b - XZB_REPS;
+				} else {
+					if (b != 0) {
+						const uint32_t d = b == 1 ? rep1 : b == 2 ? rep2 : rep3;
+						if (b == 3) rep3 = rep2;
+						if (b >= 2) rep2 = rep1;
+						rep1 = rep0; rep0 = d;
+					}
+					state = l == 1 ? (hi ? 11 : 9) : (hi ? 11 : 8);
+				}
+			}
+			const bool lit = back == XZB_BACK_LITERAL, is_m = !lit && back >= XZB_REPS;
+			n_symbols += nw;
+			match_price_count += __popc(__ballot_sync(WFULL, v && is_m));
+			align_price_count += __popc(__ballot_sync(WFULL, v && is_m && xzb_dist_slot(back - XZB_REPS) >= XZB_DIST_MODEL_END));
+			// length_count of every length in the window: k-th decrement of a counter that starts at c0, refreshed at 0
+			const bool has_len = v && !lit && (is_m || len != 1);
+			const uint32_t ci = (is_m ? 0u : XZB_POS_STATES_MAX) + ps;
+			const uint32_t grp = __match_any_sync(WFULL, has_len ? ci : 0x100u + lane);
+			const uint32_t c0 = has_len ? len_ctr[ci] : 1u, L = len_table_size;
+			const uint32_t kd = __popc(grp & lt) + 1;
+			const bool refresh = has_len && kd >= c0 && (kd - c0) % L == 0;
+			__syncwarp();
+			if (has_len && (grp >> lane) == 1) {
+				const uint32_t K = __popc(grp);
+				len_ctr[ci] = K < c0 ? c0 - K : L - (K - c0) % L;
+			}
+			if (trace != nullptr && v && trace_n + lane < trace_cap) { const uint32_t t = 3 * (trace_n + lane); trace[t] = pos + lx; trace[t + 1] = back; trace[t + 2] = len; }
+			trace_n += nw;
+			// every lane writes its symbol's records (idx | bit << 14 | direct << 15) in encode_symbol's order
+			if (v) {
+				uint16_t *const o = stg + bx;
+				const uint32_t ism = PI_IS_MATCH + (st << 4) + ps;
+				if (lit) {   // encode_literal
+					const uint32_t p = p0 + off + lx, cb = buf[p];
+					const uint32_t mb = st >= XZB_LIT_STATES ? buf[p - r0 - 1] : 0u;
+					const uint32_t sub = PI_LITERAL + 3u * (((((pos + lx) << 8) + buf[p - 1]) & literal_mask) << lc);
+					o[0] = (uint16_t)ism;
+#pragma unroll
+					for (uint32_t j = 0; j < 8; ++j) {
+						const uint32_t pre = (cb | 0x100) >> (8 - j), bit = (cb >> (7 - j)) & 1;
+						uint32_t idx = sub + pre;
+						if (st >= XZB_LIT_STATES) {
+							const uint32_t mo = ((cb ^ mb) >> (8 - j)) == 0 ? 0x100u : 0u;
+							idx += mo + (((mb >> (7 - j)) & 1) ? mo : 0u);
+						}
+						o[1 + j] = (uint16_t)(idx | (bit << 14));
+					}
+				} else {     // the prefix of encode_symbol's match / rep match, then encode_len_dist
+					const uint32_t pre_n = is_m ? 2u : (back <= 1 ? 4u : 5u);
+					o[0] = (uint16_t)(ism | (1u << 14));
+					o[1] = (uint16_t)((PI_IS_REP + st) | (is_m ? 0u : 1u << 14));
+					if (!is_m) {
+						o[2] = (uint16_t)((PI_IS_REP0 + st) | (back != 0 ? 1u << 14 : 0u));
+						o[3] = (uint16_t)(back == 0 ? (PI_IS_REP0_LONG + ism - PI_IS_MATCH) | (len != 1 ? 1u << 14 : 0u) : (PI_IS_REP1 + st) | (back != 1 ? 1u << 14 : 0u));
+						if (back >= 2) o[4] = (uint16_t)((PI_IS_REP2 + st) | ((back - 2) << 14));
+					}
+					if (nb > pre_n) {
+						const LenDist d(pre_n, is_m ? 0u : 1u, ps, len, is_m ? back - XZB_REPS : 0xFFFFFFFFu);
+						for (uint32_t k = pre_n; k < nb; ++k) {
+							uint32_t idx = 0, bit = 0;
+							const bool dr = d.at(k, idx, bit);
+							o[k] = (uint16_t)(idx | (bit << 14) | (dr ? 1u << 15 : 0u));
+						}
+					}
+				}
+			}
+			__syncwarp();
+			// then 32 records at a time, in coding order
+			const uint32_t last = nw - 1;
+			const uint32_t total = __shfl_sync(WFULL, bx + nb, last);
+			uint32_t rmask = __ballot_sync(WFULL, refresh);
+			uint32_t next = rmask ? __shfl_sync(WFULL, bx, __ffs((int)rmask) - 1) : total;   // first record of the next refresh symbol
+			for (uint32_t r = 0;;) {
+				while (rmask && next == r) {   // the refresh comes before that symbol's records
+					const uint32_t j = (uint32_t)__ffs((int)rmask) - 1;
+					rmask &= rmask - 1;
+					length_update_prices(__shfl_sync(WFULL, is_m ? 0u : 1u, j), __shfl_sync(WFULL, ps, j));
+					next = rmask ? __shfl_sync(WFULL, bx, __ffs((int)rmask) - 1) : total;
+					if (lane == 0) DP_CNT(41);
+				}
+				if (r >= total) break;
+				const uint32_t e = xzb_min(r + 32, next);
+				const bool live = r + lane < e;
+				const uint32_t w = live ? stg[r + lane] : 0x8000u;
+				const bool direct = (w & 0x8000u) != 0;
+				const uint32_t idx = w & 0x3FFFu, bit = (w >> 14) & 1;
+				// equal indices: the value before adaptation is handed on in coding (= lane) order
+				const uint32_t g = __match_any_sync(WFULL, direct ? 0x10000u + lane : idx);
+				uint32_t pv = direct ? 0u : S.probs[idx];
+				const uint32_t below = g & lt, rank = __popc(below);
+				const uint32_t pred = below ? 31u - __clz(below) : lane;
+				const uint32_t maxr = __reduce_max_sync(WFULL, rank);
+				for (uint32_t t = 1; t <= maxr; ++t) {
+					const uint32_t a = __shfl_sync(WFULL, bit ? pv - (pv >> 5) : pv + ((2048 - pv) >> 5), pred);
+					if (rank == t) pv = a;
+				}
+				if (!direct && (g >> lane) == 1) S.probs[idx] = (xzb_prob)(bit ? pv - (pv >> 5) : pv + ((2048 - pv) >> 5));
+#ifdef XZB_DP_PROF
+				if (rq_head + 32u - S.rcq_tail > DP_RCQ) {
+					DP_T(q0);
+					while (rq_head + 32u - S.rcq_tail > DP_RCQ) { }
+					DP_T(q1);
+					if (lane == 0) DP_ACC(38, q0, q1);
+				}
+#endif
+				while (rq_head + 32u - S.rcq_tail > DP_RCQ) { }   // ring space for the window
+				if (live) S.rcq[(rq_head + lane) & (DP_RCQ - 1)] = (uint16_t)(direct ? 0x2000u | (bit << 12) : pv | (bit << 12));
+				rc_run(e - r);
+				r = e;
+			}
+			if (lane == 0) DP_ACC(37, 0, total);
+			const uint32_t wl = __shfl_sync(WFULL, lx + len, last);
+			off += wl; nrec += total; done += nw;
+		}
+		read_ahead -= off;
+		uncomp_size += off;
+		sym_cur = s0 + done;
+		if (cut && lane == 0) DP_CNT(39);
+	}
+
 	// ---- lzma_lzma_encode for one LZMA2 chunk (lzma_encoder.c:266-436) ----
 	__device__ void encode_chunk(uint32_t limit)
 	{
@@ -607,6 +792,7 @@ struct DpEnc : WarpEncT<DS> {
 			is_initialized = 1;
 		}
 		for (;;) {
+			DP_T(l0);
 			if (read_pos - read_ahead >= limit || rc_pending_reaches(XZB_LZMA2_CHUNK_MAX - XZB_LOOP_INPUT_MAX)) break;
 			if (read_pos >= size) { if (read_ahead == 0) break; }
 			if (mf_stalled) break;
@@ -620,14 +806,29 @@ struct DpEnc : WarpEncT<DS> {
 #endif
 			while (rq_head - S.rcq_tail > DP_RCQ - 128u) { }   // ring space for one symbol
 			uint32_t len, back;
+			const bool fresh = sym_cur == sym_end;   // no symbols stacked: optimum_normal decides, maybe by a DP
 			DP_T(e0);
 			optimum_normal(&back, &len, uncomp_size);
 			DP_T(e1);
 			if (mf_stalled) break;
+			if (fresh && sym_cur != sym_end) {   // a DP stacked a run behind this symbol
+#ifdef XZB_DP_PROF
+				const uint32_t n0 = n_symbols;
+#endif
+				encode_batch(limit);
+#ifdef XZB_DP_PROF
+				DP_T(e2);
+				if (lane == 0 && blockIdx.x == 0) { DP_ACC(42, l0, e0); DP_ACC(13, e0, e1); DP_ACC(35, e1, e2); DP_CNT(36); S.prof[15] += n_symbols - n0; }
+#endif
+				continue;
+			}
+#ifdef XZB_DP_PROF
+			if (!fresh && lane == 0) DP_CNT(40);   // a stacked symbol left over by a cut batch
+#endif
 			if (trace != nullptr && lane == 0 && trace_n < trace_cap) { trace[3 * trace_n] = uncomp_size; trace[3 * trace_n + 1] = back; trace[3 * trace_n + 2] = len; }
 			++trace_n;
 			encode_symbol(back, len, uncomp_size);
-			{ DP_T(e2); if (lane == 0) { DP_ACC(13, e0, e1); DP_ACC(14, e1, e2); DP_CNT(15); } }
+			{ DP_T(e2); if (lane == 0) { DP_ACC(42, l0, e0); DP_ACC(13, e0, e1); DP_ACC(14, e1, e2); DP_CNT(15); DP_CNT(43); } }
 			uncomp_size += len;
 		}
 		rc_flush();

@@ -91,7 +91,7 @@ struct WarpEncT {
 		return price;
 	}
 
-	// length_update_prices (lzma_encoder.c:76-102): one lane per table entry
+	// length_update_prices (lzma_encoder.c:76-102): one lane per table entry; the caller resets the counter
 	__device__ void length_update_prices(uint32_t which, uint32_t pos_state)
 	{
 		const uint32_t base = which ? PI_REP_LEN : PI_MATCH_LEN;
@@ -104,7 +104,6 @@ struct WarpEncT {
 			else v = b1 + pr_tree(base + LC_HIGH, 8, i - XZB_LEN_LOW - XZB_LEN_MID);
 			S.len_prices[which][pos_state][i] = v;
 		}
-		if (lane == 0) S.len_counters[which][pos_state] = len_table_size;
 		__syncwarp();
 	}
 
@@ -148,7 +147,10 @@ struct WarpEncT {
 		state = 0; rep0 = rep1 = rep2 = rep3 = 0;
 		if constexpr (!FAST)
 			for (uint32_t w = 0; w < 2; ++w)
-				for (uint32_t ps = 0; ps < num_pos_states; ++ps) length_update_prices(w, ps);
+				for (uint32_t ps = 0; ps < num_pos_states; ++ps) {
+					length_update_prices(w, ps);
+					if (lane == 0) S.len_counters[w][ps] = len_table_size;
+				}
 		match_price_count = 0xFFFFFFFFu / 2;
 		align_price_count = 0xFFFFFFFFu / 2;
 	}
@@ -505,51 +507,67 @@ struct WarpEncT {
 			const uint32_t c = S.len_counters[which][pos_state] - 1;
 			__syncwarp();
 			if (c == 0) length_update_prices(which, pos_state);
-			else { if (lane == 0) S.len_counters[which][pos_state] = c; __syncwarp(); }
+			if (lane == 0) S.len_counters[which][pos_state] = c == 0 ? len_table_size : c;
+			__syncwarp();
 		}
 	}
+	// The bits of "pre_n prefix bits, then a length, then (matches) a distance" in closed form: bit k >= pre_n of the
+	// symbol, n bits in all.  dist == 0xFFFFFFFF: no distance (rep match).
+	struct LenDist {
+		uint32_t lbase, lenx, tb, tbits, lv, slot, dbase, reduced, nd, dsb, o1, o2, o3, o4, n;
+		__device__ __forceinline__ LenDist(uint32_t pre_n, uint32_t which, uint32_t pos_state, uint32_t len, uint32_t dist)
+		{
+			lbase = which ? PI_REP_LEN : PI_MATCH_LEN;
+			lenx = len - XZB_MATCH_LEN_MIN;
+			uint32_t nch;   // choice bits, the tree, its depth, the value in it
+			if (lenx < XZB_LEN_LOW) { nch = 1; tb = lbase + LC_LOW + pos_state * 8; tbits = 3; lv = lenx; }
+			else if (lenx < XZB_LEN_LOW + XZB_LEN_MID) { nch = 2; tb = lbase + LC_MID + pos_state * 8; tbits = 3; lv = lenx - XZB_LEN_LOW; }
+			else { nch = 2; tb = lbase + LC_HIGH; tbits = 8; lv = lenx - XZB_LEN_LOW - XZB_LEN_MID; }
+			o1 = pre_n; o2 = o1 + nch; o3 = o2 + tbits;
+			n = o3; slot = 0; dbase = 0; reduced = 0; nd = 0; o4 = o3;
+			if (dist != 0xFFFFFFFFu) {
+				slot = xzb_dist_slot(dist);
+				o4 = o3 + 6; n = o4;
+				if (slot >= XZB_DIST_MODEL_START) {
+					const uint32_t fb = (slot >> 1) - 1;
+					dbase = (2 | (slot & 1)) << fb;
+					reduced = dist - dbase;
+					nd = slot < XZB_DIST_MODEL_END ? 0 : fb - XZB_ALIGN_BITS;
+					n = o4 + fb;
+				}
+			}
+			dsb = PI_DIST_SLOT + xzb_dist_state(len) * 64;
+		}
+		// bit k (pre_n <= k < n): returns true for a direct bit (idx unused)
+		__device__ __forceinline__ bool at(uint32_t k, uint32_t &idx, uint32_t &bit) const
+		{
+			if (k < o2) { const uint32_t j = k - o1; idx = lbase + (j == 0 ? LC_CHOICE : LC_CHOICE2); bit = j == 0 ? (lenx >= XZB_LEN_LOW) : (lenx >= XZB_LEN_LOW + XZB_LEN_MID); }
+			else if (k < o3) bt_at(tb, tbits, lv, k - o2, idx, bit);
+			else if (k < o4) bt_at(dsb, 6, slot, k - o3, idx, bit);
+			else if (nd == 0 && slot < XZB_DIST_MODEL_END) rt_at(PI_DIST_SPECIAL + dbase - slot - 1, reduced, k - o4, idx, bit);
+			else if (k - o4 < nd) { bit = ((reduced >> XZB_ALIGN_BITS) >> (nd - 1 - (k - o4))) & 1; return true; }
+			else rt_at(PI_DIST_ALIGN, reduced & XZB_ALIGN_MASK, k - o4 - nd, idx, bit);
+			return false;
+		}
+	};
 	// Lane k's bit of "prefix bits, then a length, then (matches) a distance".  pre_n prefix bits are given by
 	// (pre_idx, pre_bit) of lane k < pre_n; dist == 0xFFFFFFFF: no distance (rep match).
 	__device__ void encode_len_dist(uint32_t pre_n, uint32_t pre_idx, uint32_t pre_bit, uint32_t which, uint32_t pos_state, uint32_t len, uint32_t dist)
 	{
-		const uint32_t lbase = which ? PI_REP_LEN : PI_MATCH_LEN;
-		const uint32_t lenx = len - XZB_MATCH_LEN_MIN;
-		uint32_t nch, tb, tbits, lv;   // choice bits, the tree, its depth, the value in it
-		if (lenx < XZB_LEN_LOW) { nch = 1; tb = lbase + LC_LOW + pos_state * 8; tbits = 3; lv = lenx; }
-		else if (lenx < XZB_LEN_LOW + XZB_LEN_MID) { nch = 2; tb = lbase + LC_MID + pos_state * 8; tbits = 3; lv = lenx - XZB_LEN_LOW; }
-		else { nch = 2; tb = lbase + LC_HIGH; tbits = 8; lv = lenx - XZB_LEN_LOW - XZB_LEN_MID; }
-		const uint32_t o1 = pre_n, o2 = o1 + nch, o3 = o2 + tbits;
-		uint32_t n = o3, slot = 0, fb = 0, dbase = 0, reduced = 0, nd = 0, o4 = o3;
-		if (dist != 0xFFFFFFFFu) {
-			slot = xzb_dist_slot(dist);
-			o4 = o3 + 6; n = o4;
-			if (slot >= XZB_DIST_MODEL_START) {
-				fb = (slot >> 1) - 1;
-				dbase = (2 | (slot & 1)) << fb;
-				reduced = dist - dbase;
-				nd = slot < XZB_DIST_MODEL_END ? 0 : fb - XZB_ALIGN_BITS;
-				n = o4 + fb;
-			}
-		}
-		const uint32_t dsb = PI_DIST_SLOT + xzb_dist_state(len) * 64;
+		const LenDist d(pre_n, which, pos_state, len, dist);
 #pragma unroll
 		for (uint32_t rnd = 0; rnd < 2; ++rnd) {
 			const uint32_t k = lane + 32 * rnd;
-			if (k < n) {
+			if (k < d.n) {
 				uint32_t idx = 0, bit = 0;
 				bool direct = false;
-				if (k < o1) { idx = pre_idx; bit = pre_bit; }
-				else if (k < o2) { const uint32_t j = k - o1; idx = lbase + (j == 0 ? LC_CHOICE : LC_CHOICE2); bit = j == 0 ? (lenx >= XZB_LEN_LOW) : (lenx >= XZB_LEN_LOW + XZB_LEN_MID); }
-				else if (k < o3) bt_at(tb, tbits, lv, k - o2, idx, bit);
-				else if (k < o4) bt_at(dsb, 6, slot, k - o3, idx, bit);
-				else if (nd == 0 && slot < XZB_DIST_MODEL_END) rt_at(PI_DIST_SPECIAL + dbase - slot - 1, reduced, k - o4, idx, bit);
-				else if (k - o4 < nd) { direct = true; bit = ((reduced >> XZB_ALIGN_BITS) >> (nd - 1 - (k - o4))) & 1; }
-				else rt_at(PI_DIST_ALIGN, reduced & XZB_ALIGN_MASK, k - o4 - nd, idx, bit);
+				if (k < d.o1) { idx = pre_idx; bit = pre_bit; }
+				else direct = d.at(k, idx, bit);
 				if (direct) rc_put_direct(k, bit);
 				else rc_put(k, idx, bit);
 			}
 		}
-		rc_run(n);
+		rc_run(d.n);
 	}
 
 	// Literal fast path of encode_symbol (lzma_encoder.c:22-69, 240-246): lane 0 = is_match bit,
