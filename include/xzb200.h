@@ -111,7 +111,7 @@ int xzb_encode_blocks_host(xzb_ctx *ctx, const uint8_t *in, uint64_t in_size,
  * ENCODE, host buffers, whole Stream: same bytes as lzma_stream_encoder_mt() +
  * lzma_code(LZMA_FINISH) (stream_encoder_mt.c:716-888, 1027-1208) with lzma_mt.block_size =
  * block_size, lzma_mt.filters = {LZMA2(opt)}, lzma_mt.check = check.
- * Host->device and device->host copies happen inside the call.
+ * Host->device and device->host copies happen inside the call.  The n = 1 case of xzb_stream_encode_batch().
  */
 int xzb_stream_encode(xzb_ctx *ctx, const uint8_t *in, uint64_t in_size,
 		const xzb_lzma_options *opt, uint32_t check, uint64_t block_size,
@@ -148,6 +148,32 @@ int xzb_stream_buffer_encode_batch(xzb_ctx *ctx, uint32_t n, const uint8_t *in, 
 /* The same with `in` and `out` in device memory (the offset / size / result arrays stay on the host). */
 int xzb_stream_buffer_encode_batch_device(xzb_ctx *ctx, uint32_t n, const uint8_t *in, const uint64_t *in_off,
 		const uint64_t *in_size, const xzb_lzma_options *opt, uint32_t check, uint8_t *out,
+		const uint64_t *out_off, const uint64_t *out_cap, uint64_t *out_size, uint32_t *ret);
+
+/*
+ * ENCODE, batch of n independent whole Streams (liblzma has no such call: this is n lzma_stream_encoder_mt() +
+ * lzma_code(LZMA_FINISH) runs at once).  Item i is in[in_off[i] .. in_off[i] + in_size[i]); its Stream is exactly what
+ * xzb_stream_encode() gives for that item alone with the same opt, check, block_size and the context's Delta/BCJ chain
+ * (xzb_ctx_set_filters): Blocks of block_size bytes framed as worker_encode() does (stream_encoder_mt.c:218-359), a
+ * multi-record Index (stream_encoder_mt.c:716-888).  It goes to out + out_off[i] (room: out_cap[i]).
+ *   - block_size == 0 is the default max(3 * dict_size, 1 MiB) (lzma2_encoder.c:403-413); block_size > 1 GiB is
+ *     XZB_OPTIONS_ERROR for the whole call.  Items have no size limit; only Blocks are capped at 1 GiB.
+ *   - ret[i] and out_size[i] are what xzb_stream_encode() gives that item alone with out_cap[i]: an item that does not
+ *     fit gets XZB_BUF_ERROR and out_size[i] = 0.  xzb_stream_bound(in_size[i], effective block_size) always suffices.
+ *   - Nothing is written outside [out_off[i], out_off[i] + out_cap[i]).  Inside the slot of a failed item the bytes are
+ *     unspecified (its Blocks are placed as their waves finish).
+ *   - n = 0, zero-length items (the 32-byte Stream: Header, an Index with no records, Footer) and unaligned offsets
+ *     are valid.
+ * The Blocks of all items are coded in waves of similar sizes, side by side on the GPU.  The return value is for errors
+ * of the whole call (options, check, device).
+ */
+int xzb_stream_encode_batch(xzb_ctx *ctx, uint32_t n, const uint8_t *in, const uint64_t *in_off,
+		const uint64_t *in_size, const xzb_lzma_options *opt, uint32_t check, uint64_t block_size, uint8_t *out,
+		const uint64_t *out_off, const uint64_t *out_cap, uint64_t *out_size, uint32_t *ret);
+/* The same with `in` and `out` in device memory (the offset / size / result arrays stay on the host).  The Stream
+ * framing is written on the GPU: no item data crosses PCIe. */
+int xzb_stream_encode_batch_device(xzb_ctx *ctx, uint32_t n, const uint8_t *in, const uint64_t *in_off,
+		const uint64_t *in_size, const xzb_lzma_options *opt, uint32_t check, uint64_t block_size, uint8_t *out,
 		const uint64_t *out_off, const uint64_t *out_cap, uint64_t *out_size, uint32_t *ret);
 
 /* Stream framing around device-encoded Blocks (stream_flags_encoder.c:29-85,

@@ -81,6 +81,9 @@ def lib():
         L.xzb_stream_buffer_encode_batch.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, P64, P64, C.POINTER(LzmaOptions), C.c_uint32,
                                                      C.c_void_p, P64, P64, P64, P32]
         L.xzb_stream_buffer_encode_batch_device.argtypes = L.xzb_stream_buffer_encode_batch.argtypes
+        L.xzb_stream_encode_batch.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, P64, P64, C.POINTER(LzmaOptions), C.c_uint32, C.c_uint64,
+                                              C.c_void_p, P64, P64, P64, P32]
+        L.xzb_stream_encode_batch_device.argtypes = L.xzb_stream_encode_batch.argtypes
         L.xzb_stream_buffer_decode_batch.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, P64, P64, C.c_void_p, P64, P64, P64, P64, P32,
                                                      C.c_uint32]
         L.xzb_stream_buffer_decode_batch_device.argtypes = L.xzb_stream_buffer_decode_batch.argtypes
@@ -202,6 +205,48 @@ class Context:
         r = lib().xzb_stream_buffer_decode(self._h, sp, len(data), out, cap, C.byref(sz), C.byref(used), flags)
         return r, bytes(out[: sz.value]), used.value
 
+    # ---- batches of independent whole Streams (xzb_stream_encode_batch[_device]) ----
+    def stream_encode_batch(self, items, preset=6, block_size=0, check=LZMA_CHECK_CRC64, opts=None, caps=None):
+        """One lzma_stream_encoder_mt Stream per item (what stream_encode gives it alone), all in one call:
+        [(ret, Stream bytes)] in item order.  caps[i] (default xzb_stream_bound of the item's size at the effective
+        Block size) is item i's output room."""
+        o = opts if opts is not None else lzma_lzma_preset(preset)
+        n = len(items)
+        views = [bytes(x) for x in items]
+        sizes = [len(v) for v in views]
+        bs = block_size if block_size else max(3 * o.dict_size, 1 << 20)
+        caps = [stream_bound(s, bs) for s in sizes] if caps is None else list(caps)
+        src = bytearray(b"".join(views)) or bytearray(1)
+        A = C.c_uint64 * max(n, 1)
+        in_off, out_off = A(), A()
+        for i in range(1, n):
+            in_off[i] = in_off[i - 1] + sizes[i - 1]
+            out_off[i] = out_off[i - 1] + caps[i - 1]
+        out = (C.c_uint8 * max(sum(caps), 1))()
+        size, rets = A(), (C.c_uint32 * max(n, 1))()
+        sp, _k = _ptr(src)
+        r = lib().xzb_stream_encode_batch(self._h, n, sp, in_off, A(*sizes), C.byref(o), check, block_size, out, out_off, A(*caps), size,
+                                          rets)
+        if r != LZMA_OK:
+            raise XzError(r, self._err())
+        raw = memoryview(out).cast("B")   # batches of several GiB: no C.string_at (its size is an int)
+        return [(rets[i], bytes(raw[out_off[i]: out_off[i] + size[i]])) for i in range(n)]
+
+    def stream_encode_batch_device(self, d_in, in_off, in_size, opts, check, block_size, d_out, out_off, out_cap):
+        """The whole-Stream batch on device memory: d_in / d_out are addresses (or CUDA tensors; synchronise their stream
+        first), the offset and size lists stay on the host.  Returns [(ret, Stream size)]; the Streams are at
+        d_out + out_off[i]."""
+        n = len(in_off)
+        A = C.c_uint64 * max(n, 1)
+        size, rets = A(), (C.c_uint32 * max(n, 1))()
+        ip, _k1 = _ptr(d_in)
+        op, _k2 = _ptr(d_out)
+        r = lib().xzb_stream_encode_batch_device(self._h, n, ip, A(*in_off), A(*in_size), C.byref(opts), check, block_size, op, A(*out_off),
+                                                 A(*out_cap), size, rets)
+        if r != LZMA_OK:
+            raise XzError(r, self._err())
+        return [(rets[i], size[i]) for i in range(n)]
+
     # ---- batches of independent one-shot Streams (xzb_stream_buffer_*_batch) ----
     def stream_buffer_encode_batch(self, items, preset=6, check=LZMA_CHECK_CRC64, opts=None, caps=None):
         """One lzma_stream_buffer_encode per item, all in one call: [(ret, Stream bytes)] in item order.
@@ -223,8 +268,8 @@ class Context:
         r = lib().xzb_stream_buffer_encode_batch(self._h, n, sp, in_off, A(*sizes), C.byref(o), check, out, out_off, A(*caps), size, rets)
         if r != LZMA_OK:
             raise XzError(r, self._err())
-        raw = C.string_at(out, len(out))
-        return [(rets[i], raw[out_off[i]: out_off[i] + size[i]]) for i in range(n)]
+        raw = memoryview(out).cast("B")   # batches of several GiB: no C.string_at (its size is an int)
+        return [(rets[i], bytes(raw[out_off[i]: out_off[i] + size[i]])) for i in range(n)]
 
     def stream_buffer_encode_batch_device(self, d_in, in_off, in_size, opts, check, d_out, out_off, out_cap):
         """The batch on device memory: d_in / d_out are addresses (or CUDA tensors; synchronise their stream first),

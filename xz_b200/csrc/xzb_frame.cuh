@@ -5,6 +5,8 @@
 // common/stream_flags_encoder.c:29-85; the read side: common/vli_decoder.c,
 // common/block_header_decoder.c, common/index_hash.c, common/stream_flags_decoder.c.
 #pragma once
+#include <vector>
+
 #include "xzb_common.cuh"
 #include "xzb_filters.cuh"
 #include "../../include/xzb200.h"
@@ -174,22 +176,21 @@ XZB_HD void xzb_block_finish_raw(const uint32_t *crc32_table, const uint8_t *in,
 }
 
 // ---- placing finished Blocks (xzb_k_pack_streams) ----
-// Size of the one-Block Stream around a Block of block_size bytes (block_size == 0: the Stream with no Block).
-XZB_HD uint64_t xzb_oneshot_stream_size(uint32_t block_size, uint64_t unpadded, uint64_t uncomp)
-{
-	return 12 + (uint64_t)block_size + xzbi_index_encode(0, &unpadded, &uncomp, block_size ? 1 : 0, 0) + 12;
-}
-
 struct alignas(16) XzbV16 { uint32_t w[4]; };
 
-// Copies the finished Block at `block` (16-byte aligned, a multiple of four bytes long) to dst; with `frame` it becomes
-// a whole one-shot Stream: Stream Header, the Block, its one-record Index, Stream Footer (stream_buffer_encoder.c:
-// 43-140).  block_size == 0 with `frame` is the Stream with no Block.  Work-shared by workers tid in [0, nthreads): the
-// Block moves in 16-byte loads; the stores are 16 bytes wide where dst allows, else 4 or 1.  Returns the bytes written.
-XZB_HD uint64_t xzb_pack_stream(const uint32_t *crc32_table, uint8_t *dst, const uint8_t *block, uint32_t block_size,
-		uint64_t unpadded, uint64_t uncomp, uint32_t check, bool frame, uint32_t tid, uint32_t nthreads)
+// Stream framing a placed Block carries: the first Block of a Stream brings the Stream Header, the last one the Index
+// and the Stream Footer (stream_encoder_mt.c:716-888; one-shot Streams, stream_buffer_encoder.c:43-140, are both).
+enum { XZB_PACK_HEAD = 1, XZB_PACK_TAIL = 2 };
+
+// Copies the finished Block at `block` (16-byte aligned, a multiple of four bytes long) to dst.  XZB_PACK_HEAD writes
+// the Stream Header into the 12 bytes before dst; XZB_PACK_TAIL writes the Index over the Stream's `count` records
+// (unpadded[k], uncomp[k]) and the Stream Footer right behind the Block.  HEAD | TAIL with block_size == 0 and
+// count == 0 is the Stream with no Block.  Work-shared by workers tid in [0, nthreads): the Block moves in 16-byte
+// loads; the stores are 16 bytes wide where dst allows, else 4 or 1.  Returns the bytes written, header included.
+XZB_HD uint64_t xzb_pack_block(const uint32_t *crc32_table, uint8_t *dst, const uint8_t *block, uint32_t block_size, uint32_t flags,
+		const uint64_t *unpadded, const uint64_t *uncomp, uint64_t count, uint32_t check, uint32_t tid, uint32_t nthreads)
 {
-	uint8_t *d = dst + (frame ? 12 : 0);
+	uint8_t *d = dst;
 	const uint32_t nv = block_size / 16;
 	const XzbV16 *src = (const XzbV16 *)block;
 	const uintptr_t da = (uintptr_t)d;
@@ -200,13 +201,56 @@ XZB_HD uint64_t xzb_pack_stream(const uint32_t *crc32_table, uint8_t *dst, const
 		else for (int k = 0; k < 16; ++k) d[16 * i + k] = (uint8_t)(v.w[k >> 2] >> (8 * (k & 3)));
 	}
 	for (uint32_t i = 16 * nv + tid; i < block_size; i += nthreads) d[i] = block[i];
-	if (!frame) return block_size;
-	if (tid == 0) {
-		xzb_stream_header(crc32_table, dst, check);
-		const uint64_t isz = xzbi_index_encode(crc32_table, &unpadded, &uncomp, block_size ? 1 : 0, d + block_size);
-		xzb_stream_footer(crc32_table, d + block_size + isz, check, isz);
+	uint64_t size = block_size;
+	if (flags & XZB_PACK_HEAD) {
+		if (tid == 0) xzb_stream_header(crc32_table, d - 12, check);
+		size += 12;
 	}
-	return xzb_oneshot_stream_size(block_size, unpadded, uncomp);
+	if (flags & XZB_PACK_TAIL) {
+		const uint64_t isz = xzbi_index_encode(crc32_table, unpadded, uncomp, count, tid == 0 ? d + block_size : nullptr);
+		if (tid == 0) xzb_stream_footer(crc32_table, d + block_size + isz, check, isz);
+		size += isz + 12;
+	}
+	return size;
+}
+
+// The one-shot form: with `frame`, the whole one-Block Stream (stream_buffer_encoder.c:43-140) starting at dst --
+// Stream Header, the Block, its one-record Index, Stream Footer; block_size == 0 is the Stream with no Block --
+// else the bare Block at dst.  Returns the bytes written.
+XZB_HD uint64_t xzb_pack_stream(const uint32_t *crc32_table, uint8_t *dst, const uint8_t *block, uint32_t block_size,
+		uint64_t unpadded, uint64_t uncomp, uint32_t check, bool frame, uint32_t tid, uint32_t nthreads)
+{
+	return xzb_pack_block(crc32_table, dst + (frame ? 12 : 0), block, block_size, frame ? XZB_PACK_HEAD | XZB_PACK_TAIL : 0, &unpadded, &uncomp,
+			frame && block_size ? 1 : 0, check, tid, nthreads);
+}
+
+// Host: placement of one Stream in its output slot as its Blocks finish, in Block order (a Block's offset is the sum
+// of the Blocks before it).  recs: Unpadded Sizes [0, nblocks), then Uncompressed Sizes [nblocks, 2 nblocks).
+struct XzbStreamPlace {
+	uint64_t cap = 0, nblocks = 0;
+	uint64_t next = 0;    // Blocks placed so far
+	uint64_t pos = 12;    // where the next Block goes; once the last one is placed, the Stream's size
+	std::vector<uint64_t> recs;
+};
+
+// Places the Stream's next Block (total_size bytes; nothing for a Stream with no Block): returns its offset in the slot
+// and, in *flags, the framing it carries -- or UINT64_MAX when it, or with the last Block the Index and the Stream
+// Footer, would cross s.cap.
+static inline uint64_t xzb_stream_place(XzbStreamPlace &s, uint32_t total_size, uint64_t unpadded, uint64_t uncomp, uint32_t *flags)
+{
+	const uint64_t at = s.pos;
+	*flags = s.next == 0 ? XZB_PACK_HEAD : 0;
+	if (s.nblocks != 0) {
+		s.recs.resize(2 * s.nblocks);
+		s.recs[s.next] = unpadded; s.recs[s.nblocks + s.next] = uncomp;
+		++s.next;
+	}
+	s.pos += total_size;
+	if (s.next == s.nblocks) {
+		*flags |= XZB_PACK_TAIL;
+		s.pos += xzbi_index_encode(nullptr, s.recs.data(), s.recs.data() + s.nblocks, s.nblocks, nullptr) + 12;
+	}
+	return s.pos <= s.cap ? at : UINT64_MAX;
 }
 
 // ---- read side (host and device), over untrusted input: every reader stays inside the `size` / `avail` bytes it is given ----

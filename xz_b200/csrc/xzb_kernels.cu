@@ -452,20 +452,22 @@ xzb_k_finalize(const XzbEncJob *__restrict__ jobs, const uint32_t *__restrict__ 
 		xzb_block_finish_raw(crc32_table, job.in, job.in_size, job.out, check, check_bytes + (size_t)b * 32, res, threadIdx.x, blockDim.x);
 }
 
-// Places finished Blocks: one CTA per job copies its Block out of scratch to `dst`; with `frame` the job becomes a whole
-// one-shot Stream (xzb_pack_stream).  src == nullptr with frame: the Stream with no Block.
+// Places finished Blocks: one CTA per job copies its Block out of scratch to `dst`, with the Stream framing `flags`
+// asks for (xzb_pack_block).  src == nullptr, size 0: the Stream with no Block.  recs: with XZB_PACK_TAIL, the
+// Stream's Unpadded Sizes [0, nrecs), then its Uncompressed Sizes.
 struct XzbPackJob {
 	const uint8_t *src;
 	uint8_t *dst;
-	uint64_t unpadded, uncomp;
-	uint32_t size, frame;
+	const uint64_t *recs;
+	uint64_t nrecs;
+	uint32_t size, flags;
 };
 
 __global__ void __launch_bounds__(256)
 xzb_k_pack_streams(const XzbPackJob *__restrict__ jobs, const uint32_t *__restrict__ crc32_table, uint32_t check)
 {
 	const XzbPackJob j = jobs[blockIdx.x];
-	xzb_pack_stream(crc32_table, j.dst, j.src, j.size, j.unpadded, j.uncomp, check, j.frame != 0, threadIdx.x, blockDim.x);
+	xzb_pack_block(crc32_table, j.dst, j.src, j.size, j.flags, j.recs, j.recs + j.nrecs, j.nrecs, check, threadIdx.x, blockDim.x);
 }
 
 // ---- Delta / BCJ filters over whole Blocks (xzb_filters.cuh) ----
@@ -1259,36 +1261,47 @@ static int encode_begin(xzb_ctx *ctx, const xzb_lzma_options *opt, uint32_t chec
 	return XZB_OK;
 }
 
-// Places finished Blocks (and, for framed jobs, whole one-shot Streams) with one xzb_k_pack_streams launch, then
+// Places finished Blocks (and the Stream framing their jobs ask for) with one xzb_k_pack_streams launch, then
 // synchronises.  host_out == nullptr: every job's dst is a device address.  Otherwise each dst is an offset into a
-// staging area of stage_bytes, which comes back to host_out with one copy.
-static int place_blocks(xzb_ctx *ctx, std::vector<XzbPackJob> &jobs, uint32_t check, uint8_t *host_out, size_t stage_bytes)
+// staging area of stage_bytes, which comes back to host_out with one copy.  A job's `recs` is an index into `recs`,
+// which goes up behind the jobs in the same copy.
+static int place_blocks(xzb_ctx *ctx, std::vector<XzbPackJob> &jobs, const std::vector<uint64_t> &recs, uint32_t check, uint8_t *host_out,
+		size_t stage_bytes)
 {
 	cudaStream_t st = ctx->stream;
+	std::vector<uint8_t> up;
 	if (!jobs.empty()) {
 		if (host_out != nullptr) {
 			EN(ctx->out_stage, stage_bytes + 64);
 			for (XzbPackJob &j : jobs) j.dst = (uint8_t *)ctx->out_stage.p + (size_t)j.dst;
 		}
-		EN(ctx->pack_jobs, sizeof(XzbPackJob) * jobs.size());
-		CK(cudaMemcpyAsync(ctx->pack_jobs.p, jobs.data(), sizeof(XzbPackJob) * jobs.size(), cudaMemcpyHostToDevice, st));
+		const size_t jobs_bytes = sizeof(XzbPackJob) * jobs.size(), recs_bytes = sizeof(uint64_t) * recs.size();
+		EN(ctx->pack_jobs, jobs_bytes + recs_bytes);
+		const uint64_t *d_recs = (const uint64_t *)((uint8_t *)ctx->pack_jobs.p + jobs_bytes);
+		for (XzbPackJob &j : jobs) j.recs = d_recs + (size_t)j.recs;
+		up.resize(jobs_bytes + recs_bytes);
+		memcpy(up.data(), jobs.data(), jobs_bytes);
+		if (recs_bytes) memcpy(up.data() + jobs_bytes, recs.data(), recs_bytes);
+		CK(cudaMemcpyAsync(ctx->pack_jobs.p, up.data(), up.size(), cudaMemcpyHostToDevice, st));
 		xzb_k_pack_streams<<<(uint32_t)jobs.size(), 256, 0, st>>>((const XzbPackJob *)ctx->pack_jobs.p, ctx->d_crc32, check);
 		++ctx->stats.gpu_launches;
 		if (host_out != nullptr && stage_bytes > 0) CK(cudaMemcpyAsync(host_out, ctx->out_stage.p, stage_bytes, cudaMemcpyDeviceToHost, st));
 	}
-	CK(cudaStreamSynchronize(st));   // also: `jobs` is the source of the copy above
+	CK(cudaStreamSynchronize(st));   // also: `up` is the source of the copy above
 	CK(cudaGetLastError());
 	return XZB_OK;
 }
 
+// lzma_lzma2_block_size, lzma2_encoder.c:403-413: the Block size lzma_stream_encoder_mt() takes for block_size == 0
+static uint64_t default_block_size(const XzbParams &P) { return std::max<uint64_t>((uint64_t)P.dict_size * 3, 1u << 20); }
+
 static int encode_common(xzb_ctx *ctx, const uint8_t *in, bool in_is_device, uint64_t in_size, const xzb_lzma_options *opt, uint32_t check,
-		uint64_t block_size, uint8_t *out, bool out_is_device, uint64_t out_cap, uint64_t *out_size, xzb_index_record *records,
-		bool whole_stream)
+		uint64_t block_size, uint8_t *out, bool out_is_device, uint64_t out_cap, uint64_t *out_size, xzb_index_record *records)
 {
 	XzbParams P;
 	int r = encode_begin(ctx, opt, check, P);
 	if (r != XZB_OK) return r;
-	if (block_size == 0) block_size = std::max<uint64_t>((uint64_t)P.dict_size * 3, 1u << 20);  // lzma_lzma2_block_size, lzma2_encoder.c:403-413
+	if (block_size == 0) block_size = default_block_size(P);
 	if (block_size > (1ull << 30)) return set_err(ctx, XZB_OPTIONS_ERROR, "block_size > 1 GiB is not supported on the GPU path");
 	const uint64_t nblocks = (in_size + block_size - 1) / block_size;
 	const uint32_t bs = (uint32_t)block_size;
@@ -1296,13 +1309,6 @@ static int encode_common(xzb_ctx *ctx, const uint8_t *in, bool in_is_device, uin
 	uint64_t pos = 0;
 	cudaStream_t st = ctx->stream;
 	CK(cudaEventRecord(ctx->ev[6], st));
-	if (whole_stream) {
-		uint8_t hdr[12];
-		xzb_stream_header(ctx->h_tab.crc32, hdr, check);
-		if (out_cap < 12) return set_err(ctx, XZB_BUF_ERROR, "output too small");
-		if (out_is_device) CK(cudaMemcpyAsync(out, hdr, 12, cudaMemcpyHostToDevice, st)); else memcpy(out, hdr, 12);
-		pos = 12;
-	}
 	uint64_t done = 0;
 	const uint64_t bound = xzbi_block_bound(block_size);
 	const uint32_t header_size = xzb_block_header_size(bound, block_size, P.ff_len);
@@ -1340,26 +1346,17 @@ static int encode_common(xzb_ctx *ctx, const uint8_t *in, bool in_is_device, uin
 			if (res.ret != XZB_OK) return set_err(ctx, (int)res.ret, "block %llu failed", (unsigned long long)(done + b));
 			if (pos + res.total_size > out_cap) return set_err(ctx, XZB_BUF_ERROR, "output buffer too small");
 			uint8_t *dst = out_is_device ? out + pos : (uint8_t *)(uintptr_t)(pos - pos0);
-			jobs[b] = XzbPackJob{ (const uint8_t *)ctx->scratch.p + sc_off[b], dst, 0, 0, res.total_size, 0 };
+			jobs[b] = XzbPackJob{ (const uint8_t *)ctx->scratch.p + sc_off[b], dst, nullptr, 0, res.total_size, 0 };
 			pos += res.total_size;
 			recs[done + b].unpadded_size = res.unpadded_size;
 			recs[done + b].uncompressed_size = wb[b].n;
 		}
-		r = place_blocks(ctx, jobs, check, out_is_device ? nullptr : out + pos0, pos - pos0);
+		r = place_blocks(ctx, jobs, {}, check, out_is_device ? nullptr : out + pos0, pos - pos0);
 		if (r != XZB_OK) return r;
 		CK(cudaEventRecord(ctx->ev[11], st));
 		CK(cudaStreamSynchronize(st));
 		if (!out_is_device) ctx->stats.ms_d2h += ev_ms(ctx->ev[10], ctx->ev[11]); else ctx->stats.ms_other += ev_ms(ctx->ev[10], ctx->ev[11]);
 		done += W;
-	}
-	if (whole_stream) {
-		const uint64_t isz = xzb_index_encode(recs.data(), nblocks, nullptr);
-		if (pos + isz + 12 > out_cap) return set_err(ctx, XZB_BUF_ERROR, "output buffer too small");
-		std::vector<uint8_t> tail(isz + 12);
-		xzb_index_encode(recs.data(), nblocks, tail.data());
-		xzb_stream_footer(ctx->h_tab.crc32, tail.data() + isz, check, isz);
-		if (out_is_device) CK(cudaMemcpyAsync(out + pos, tail.data(), tail.size(), cudaMemcpyHostToDevice, st)); else memcpy(out + pos, tail.data(), tail.size());
-		pos += tail.size();
 	}
 	CK(cudaEventRecord(ctx->ev[7], st));
 	CK(cudaStreamSynchronize(st));
@@ -1372,19 +1369,13 @@ static int encode_common(xzb_ctx *ctx, const uint8_t *in, bool in_is_device, uin
 extern "C" int xzb_encode_blocks_device(xzb_ctx *ctx, const void *d_in, uint64_t in_size, const xzb_lzma_options *opt, uint32_t check,
 		uint64_t block_size, void *d_out, uint64_t d_out_cap, uint64_t *out_size, xzb_index_record *records)
 {
-	return encode_common(ctx, (const uint8_t *)d_in, true, in_size, opt, check, block_size, (uint8_t *)d_out, true, d_out_cap, out_size, records, false);
+	return encode_common(ctx, (const uint8_t *)d_in, true, in_size, opt, check, block_size, (uint8_t *)d_out, true, d_out_cap, out_size, records);
 }
 
 extern "C" int xzb_encode_blocks_host(xzb_ctx *ctx, const uint8_t *in, uint64_t in_size, const xzb_lzma_options *opt, uint32_t check,
 		uint64_t block_size, uint8_t *out, uint64_t out_cap, uint64_t *out_size, xzb_index_record *records)
 {
-	return encode_common(ctx, in, false, in_size, opt, check, block_size, out, false, out_cap, out_size, records, false);
-}
-
-extern "C" int xzb_stream_encode(xzb_ctx *ctx, const uint8_t *in, uint64_t in_size, const xzb_lzma_options *opt, uint32_t check,
-		uint64_t block_size, uint8_t *out, uint64_t out_cap, uint64_t *out_size)
-{
-	return encode_common(ctx, in, false, in_size, opt, check, block_size, out, false, out_cap, out_size, nullptr, true);
+	return encode_common(ctx, in, false, in_size, opt, check, block_size, out, false, out_cap, out_size, records);
 }
 
 // A Block with no uncompressed data, as lzma_block_buffer_encode() produces it for in_size == 0
@@ -1416,90 +1407,144 @@ extern "C" uint64_t xzb_stream_buffer_bound(uint64_t in_size)
 	return bb + hb;
 }
 
-// n independent one-shot Streams.  The items are encoded in waves of similar sizes (xzb_plan_waves), each Block framed
-// as lzma_block_buffer_encode() does (block_encode_normal(), block_buffer_encoder.c:165-183: header sized from
-// lzma2_bound(n), the LZMA2 data alone must fit) and turned into its Stream by xzb_k_pack_streams.
+// n independent Streams, the Blocks of all of them coded in shared waves (xzb_plan_waves) and placed, with their
+// Stream framing, by xzb_k_pack_streams.  Two framings:
+//   whole == false  one-shot Streams: each item is ONE Block framed as lzma_block_buffer_encode() does
+//                   (block_encode_normal(), block_buffer_encoder.c:165-183: header sized from lzma2_bound(n), the
+//                   LZMA2 data alone must fit), items up to 1 GiB;
+//   whole == true   lzma_stream_encoder_mt() Streams: each item is cut into Blocks of block_size framed as
+//                   worker_encode() does (stream_encoder_mt.c:218-359, as encode_common: every Block's header is sized
+//                   from lzma_block_buffer_bound64(block_size), the short last one's too, and the whole Block must fit
+//                   that bound), items of any size.
 static int encode_batch(xzb_ctx *ctx, uint32_t n, const uint8_t *in, bool in_is_device, const uint64_t *in_off, const uint64_t *in_size,
-		const xzb_lzma_options *opt, uint32_t check, uint8_t *out, bool out_is_device, const uint64_t *out_off, const uint64_t *out_cap,
-		uint64_t *out_size, uint32_t *ret)
+		const xzb_lzma_options *opt, uint32_t check, bool whole, uint64_t block_size, uint8_t *out, bool out_is_device,
+		const uint64_t *out_off, const uint64_t *out_cap, uint64_t *out_size, uint32_t *ret)
 {
 	XzbParams P;
 	int r = encode_begin(ctx, opt, check, P);
 	if (r != XZB_OK) return r;
+	if (whole && block_size == 0) block_size = default_block_size(P);
+	if (whole && block_size > (1ull << 30)) return set_err(ctx, XZB_OPTIONS_ERROR, "block_size > 1 GiB is not supported on the GPU path");
+	const uint64_t whole_bound = xzbi_block_bound(block_size);
+	const uint32_t whole_hs = xzb_block_header_size(whole_bound, block_size, P.ff_len);
 	cudaStream_t st = ctx->stream;
 	CK(cudaEventRecord(ctx->ev[6], st));
-	std::vector<uint32_t> items;       // the items with a Block
+	// Every Block of every item, in (item, j) order: Block j of item i is in_size[i] bytes from j * block_size on.
+	struct Blk { uint32_t item; uint64_t j, start; };
+	std::vector<Blk> blks;
 	std::vector<uint64_t> sizes;
-	std::vector<XzbPackJob> empties;   // Streams with no Block
-	std::vector<uint32_t> empty_items;
+	std::vector<XzbStreamPlace> place(n);
+	std::vector<uint32_t> no_block;   // items whose Stream has no Block
 	for (uint32_t i = 0; i < n; ++i) {
 		out_size[i] = 0; ret[i] = XZB_OK;
-		if (in_size[i] > (1ull << 30)) { ret[i] = XZB_OPTIONS_ERROR; set_err(ctx, XZB_OPTIONS_ERROR, "block_size > 1 GiB is not supported on the GPU path"); }
-		else if (in_size[i] == 0) { empty_items.push_back(i); }
-		else { items.push_back(i); sizes.push_back(in_size[i]); }
-	}
-	// Host output goes through a staging area packed in call order of the items that fit, then back in one copy.
-	std::vector<uint8_t> host_stage;
-	auto place = [&](const std::vector<uint32_t> &who, std::vector<XzbPackJob> &jobs) -> int {
-		uint64_t stage = 0;
-		std::vector<XzbPackJob> keep;
-		std::vector<uint32_t> kept;
-		for (size_t k = 0; k < jobs.size(); ++k) {
-			const uint32_t i = who[k];
-			const uint64_t size = xzb_oneshot_stream_size(jobs[k].size, jobs[k].unpadded, jobs[k].uncomp);
-			if (size > out_cap[i]) { ret[i] = XZB_BUF_ERROR; set_err(ctx, XZB_BUF_ERROR, "output buffer too small"); continue; }
-			out_size[i] = size;
-			jobs[k].dst = out_is_device ? out + out_off[i] : (uint8_t *)(uintptr_t)stage;
-			stage += (size + 15) & ~15ull;
-			keep.push_back(jobs[k]); kept.push_back(i);
+		place[i].cap = out_cap[i];
+		if (!whole && in_size[i] > (1ull << 30)) { ret[i] = XZB_OPTIONS_ERROR; set_err(ctx, XZB_OPTIONS_ERROR, "block_size > 1 GiB is not supported on the GPU path"); continue; }
+		if (in_size[i] == 0) { no_block.push_back(i); continue; }
+		const uint64_t bs = whole ? block_size : in_size[i];
+		place[i].nblocks = (in_size[i] + bs - 1) / bs;
+		for (uint64_t j = 0; j < place[i].nblocks; ++j) {
+			blks.push_back(Blk{ i, j, j * bs });
+			sizes.push_back(std::min(bs, in_size[i] - j * bs));
 		}
+	}
+	// Pack jobs of the Blocks placed so far and, for host output, where each piece (a Block with the framing its job
+	// writes around it) sits in the staging area and in its item's slot.
+	std::vector<XzbPackJob> jobs;
+	std::vector<uint64_t> recs;
+	struct Piece { uint32_t item; uint64_t from, len, stage; };
+	std::vector<Piece> pieces;
+	uint64_t stage = 0;
+	std::vector<uint8_t> host_stage;
+	auto add_job = [&](uint32_t i, uint64_t at, uint32_t flags, const uint8_t *src, uint32_t size) {
+		const XzbStreamPlace &s = place[i];
+		const uint64_t from = at - ((flags & XZB_PACK_HEAD) ? 12 : 0), to = (flags & XZB_PACK_TAIL) ? s.pos : at + size;
+		uint8_t *dst = out + out_off[i] + at;
+		if (!out_is_device) {
+			dst = (uint8_t *)(uintptr_t)(stage + (at - from));
+			pieces.push_back(Piece{ i, from, to - from, stage });
+			stage += (to - from + 15) & ~15ull;
+		}
+		uint64_t rec_at = 0, nrecs = 0;
+		if (flags & XZB_PACK_TAIL) {
+			rec_at = recs.size(); nrecs = s.nblocks;
+			recs.insert(recs.end(), s.recs.begin(), s.recs.end());
+			out_size[i] = s.pos;
+		}
+		jobs.push_back(XzbPackJob{ src, dst, (const uint64_t *)(uintptr_t)rec_at, nrecs, size, flags });
+	};
+	auto flush = [&]() -> int {
+		CK(cudaEventRecord(ctx->ev[10], st));
 		if (!out_is_device) host_stage.resize(stage);
-		const int pr = place_blocks(ctx, keep, check, out_is_device ? nullptr : host_stage.data(), stage);
+		const int pr = place_blocks(ctx, jobs, recs, check, out_is_device ? nullptr : host_stage.data(), stage);
 		if (pr != XZB_OK) return pr;
-		if (!out_is_device)
-			for (size_t k = 0; k < keep.size(); ++k)
-				memcpy(out + out_off[kept[k]], host_stage.data() + (keep[k].dst - (uint8_t *)ctx->out_stage.p), out_size[kept[k]]);
+		for (const Piece &p : pieces) memcpy(out + out_off[p.item] + p.from, host_stage.data() + p.stage, p.len);
+		CK(cudaEventRecord(ctx->ev[11], st));
+		CK(cudaStreamSynchronize(st));
+		if (!out_is_device) ctx->stats.ms_d2h += ev_ms(ctx->ev[10], ctx->ev[11]); else ctx->stats.ms_other += ev_ms(ctx->ev[10], ctx->ev[11]);
+		jobs.clear(); recs.clear(); pieces.clear(); stage = 0;
 		return XZB_OK;
 	};
+	// xzb_plan_waves sorts stably, largest first, and every Block of an item but its last is block_size long: so an
+	// item's Blocks keep their j order, and all Blocks before Block j are in its wave or an earlier one.  Placement
+	// (Block j at the sum of the sizes of Blocks 0 .. j-1) relies on that.
 	const uint32_t hbm = bit_length(P.hash_mask);
 	std::vector<uint32_t> order, wave_start;
 	xzb_plan_waves(sizes.data(), (uint32_t)sizes.size(), xzb_wave_cost(P), wave_budget(ctx, 0), hbm, ctx->max_wave_blocks, &order, &wave_start);
 	for (size_t w = 0; w + 1 < wave_start.size(); ++w) {
 		const uint32_t B = wave_start[w + 1] - wave_start[w];
-		std::vector<uint32_t> who(B), wn(B), woff(B);
-		for (uint32_t b = 0; b < B; ++b) { who[b] = items[order[wave_start[w] + b]]; wn[b] = (uint32_t)in_size[who[b]]; }
+		const uint32_t *ord = order.data() + wave_start[w];
+		std::vector<uint32_t> wn(B), woff(B);
+		for (uint32_t b = 0; b < B; ++b) wn[b] = (uint32_t)sizes[ord[b]];
 		// the wave's inputs side by side in HBM, each at its Block's workspace offset; the 64 bytes behind the last one
 		// are the slack the match finder may read past every Block
 		const uint64_t total = xzb_wave_offsets(wn.data(), B, woff.data());
 		EN(ctx->in_stage, total + 64);
 		uint8_t *d_wave = (uint8_t *)ctx->in_stage.p;
 		CK(cudaEventRecord(ctx->ev[8], st));
-		for (uint32_t b = 0; b < B; ++b)
-			CK(cudaMemcpyAsync(d_wave + woff[b], in + in_off[who[b]], wn[b], in_is_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, st));
+		for (uint32_t b = 0; b < B; ++b) {
+			const Blk &k = blks[ord[b]];
+			CK(cudaMemcpyAsync(d_wave + woff[b], in + in_off[k.item] + k.start, wn[b], in_is_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, st));
+		}
 		CK(cudaEventRecord(ctx->ev[9], st));
+		// Scratch is sized from the Block's own length, not from block_size: LZMA2 data never exceeds lzma2_bound(n)
+		// (the chunker stores a chunk uncompressed once it does not shrink), which is below xzb_scratch_cap(n), so the
+		// chunker never stops short of it and the bytes are those a block_size scratch would give.
 		std::vector<XzbWaveBlock> wb(B);
 		for (uint32_t b = 0; b < B; ++b) {
-			const uint32_t hs = xzb_block_header_size(xzb_lzma2_bound(wn[b]), wn[b], P.ff_len);
-			wb[b] = XzbWaveBlock{ woff[b], wn[b], wn[b] + 8, hs, 1, hs + xzb_lzma2_bound(wn[b]), xzb_scratch_cap(wn[b]) };
+			if (whole) {
+				wb[b] = XzbWaveBlock{ woff[b], wn[b], wn[b] + 8, whole_hs, 0, whole_bound, xzb_scratch_cap(wn[b]) };
+			} else {
+				const uint32_t hs = xzb_block_header_size(xzb_lzma2_bound(wn[b]), wn[b], P.ff_len);
+				wb[b] = XzbWaveBlock{ woff[b], wn[b], wn[b] + 8, hs, 1, hs + xzb_lzma2_bound(wn[b]), xzb_scratch_cap(wn[b]) };
+			}
 		}
 		std::vector<XzbBlockResult> results;
 		std::vector<size_t> sc_off;
 		r = encode_wave(ctx, d_wave, total, wb, P, check, results, sc_off);
 		if (r != XZB_OK) return r;
 		ctx->stats.ms_h2d += ev_ms(ctx->ev[8], ctx->ev[9]);
-		std::vector<XzbPackJob> jobs;
-		std::vector<uint32_t> placed;
 		for (uint32_t b = 0; b < B; ++b) {
+			const Blk &k = blks[ord[b]];
 			const XzbBlockResult &res = results[b];
-			if (res.ret != XZB_OK) { ret[who[b]] = res.ret; set_err(ctx, (int)res.ret, "item %u failed", who[b]); continue; }
-			jobs.push_back(XzbPackJob{ (const uint8_t *)ctx->scratch.p + sc_off[b], nullptr, res.unpadded_size, wn[b], res.total_size, 1 });
-			placed.push_back(who[b]);
+			XzbStreamPlace &s = place[k.item];
+			if (ret[k.item] != XZB_OK) continue;
+			if (res.ret != XZB_OK) { ret[k.item] = res.ret; set_err(ctx, (int)res.ret, "item %u failed", k.item); continue; }
+			if (k.j != s.next) return set_err(ctx, XZB_PROG_ERROR, "Block %llu of item %u placed out of order", (unsigned long long)k.j, k.item);
+			uint32_t flags;
+			const uint64_t at = xzb_stream_place(s, res.total_size, res.unpadded_size, wn[b], &flags);
+			if (at == UINT64_MAX) { ret[k.item] = XZB_BUF_ERROR; set_err(ctx, XZB_BUF_ERROR, "output buffer too small"); continue; }
+			add_job(k.item, at, flags, (const uint8_t *)ctx->scratch.p + sc_off[b], res.total_size);
 		}
-		r = place(placed, jobs);
+		r = flush();
 		if (r != XZB_OK) return r;
 	}
-	for (size_t k = 0; k < empty_items.size(); ++k) empties.push_back(XzbPackJob{ nullptr, nullptr, 0, 0, 0, 1 });
-	r = place(empty_items, empties);
+	for (const uint32_t i : no_block) {
+		uint32_t flags;
+		const uint64_t at = xzb_stream_place(place[i], 0, 0, 0, &flags);
+		if (at == UINT64_MAX) { ret[i] = XZB_BUF_ERROR; set_err(ctx, XZB_BUF_ERROR, "output buffer too small"); continue; }
+		add_job(i, at, flags, nullptr, 0);
+	}
+	r = flush();
 	if (r != XZB_OK) return r;
 	CK(cudaEventRecord(ctx->ev[7], st));
 	CK(cudaStreamSynchronize(st));
@@ -1510,13 +1555,13 @@ static int encode_batch(xzb_ctx *ctx, uint32_t n, const uint8_t *in, bool in_is_
 extern "C" int xzb_stream_buffer_encode_batch(xzb_ctx *ctx, uint32_t n, const uint8_t *in, const uint64_t *in_off, const uint64_t *in_size,
 		const xzb_lzma_options *opt, uint32_t check, uint8_t *out, const uint64_t *out_off, const uint64_t *out_cap, uint64_t *out_size, uint32_t *ret)
 {
-	return encode_batch(ctx, n, in, false, in_off, in_size, opt, check, out, false, out_off, out_cap, out_size, ret);
+	return encode_batch(ctx, n, in, false, in_off, in_size, opt, check, false, 0, out, false, out_off, out_cap, out_size, ret);
 }
 
 extern "C" int xzb_stream_buffer_encode_batch_device(xzb_ctx *ctx, uint32_t n, const uint8_t *in, const uint64_t *in_off, const uint64_t *in_size,
 		const xzb_lzma_options *opt, uint32_t check, uint8_t *out, const uint64_t *out_off, const uint64_t *out_cap, uint64_t *out_size, uint32_t *ret)
 {
-	return encode_batch(ctx, n, in, true, in_off, in_size, opt, check, out, true, out_off, out_cap, out_size, ret);
+	return encode_batch(ctx, n, in, true, in_off, in_size, opt, check, false, 0, out, true, out_off, out_cap, out_size, ret);
 }
 
 extern "C" int xzb_stream_buffer_encode(xzb_ctx *ctx, const uint8_t *in, uint64_t in_size, const xzb_lzma_options *opt, uint32_t check,
@@ -1525,7 +1570,33 @@ extern "C" int xzb_stream_buffer_encode(xzb_ctx *ctx, const uint8_t *in, uint64_
 	const uint64_t zero = 0;
 	uint64_t size = 0;
 	uint32_t ret = XZB_OK;
-	const int r = encode_batch(ctx, 1, in, false, &zero, &in_size, opt, check, out, false, &zero, &out_cap, &size, &ret);
+	const int r = encode_batch(ctx, 1, in, false, &zero, &in_size, opt, check, false, 0, out, false, &zero, &out_cap, &size, &ret);
+	if (r != XZB_OK) return r;
+	if (ret == XZB_OK) *out_size = size;
+	return (int)ret;
+}
+
+extern "C" int xzb_stream_encode_batch(xzb_ctx *ctx, uint32_t n, const uint8_t *in, const uint64_t *in_off, const uint64_t *in_size,
+		const xzb_lzma_options *opt, uint32_t check, uint64_t block_size, uint8_t *out, const uint64_t *out_off, const uint64_t *out_cap,
+		uint64_t *out_size, uint32_t *ret)
+{
+	return encode_batch(ctx, n, in, false, in_off, in_size, opt, check, true, block_size, out, false, out_off, out_cap, out_size, ret);
+}
+
+extern "C" int xzb_stream_encode_batch_device(xzb_ctx *ctx, uint32_t n, const uint8_t *in, const uint64_t *in_off, const uint64_t *in_size,
+		const xzb_lzma_options *opt, uint32_t check, uint64_t block_size, uint8_t *out, const uint64_t *out_off, const uint64_t *out_cap,
+		uint64_t *out_size, uint32_t *ret)
+{
+	return encode_batch(ctx, n, in, true, in_off, in_size, opt, check, true, block_size, out, true, out_off, out_cap, out_size, ret);
+}
+
+extern "C" int xzb_stream_encode(xzb_ctx *ctx, const uint8_t *in, uint64_t in_size, const xzb_lzma_options *opt, uint32_t check,
+		uint64_t block_size, uint8_t *out, uint64_t out_cap, uint64_t *out_size)
+{
+	const uint64_t zero = 0;
+	uint64_t size = 0;
+	uint32_t ret = XZB_OK;
+	const int r = encode_batch(ctx, 1, in, false, &zero, &in_size, opt, check, true, block_size, out, false, &zero, &out_cap, &size, &ret);
 	if (r != XZB_OK) return r;
 	if (ret == XZB_OK) *out_size = size;
 	return (int)ret;
