@@ -255,6 +255,40 @@ int xzb_decode_blocks_device(xzb_ctx *ctx, const void *d_in, const uint64_t *com
 		const uint32_t *dict_size, uint32_t nblocks, uint32_t check, void *d_out,
 		uint32_t *ret, uint64_t *check_out);
 
+/*
+ * DECODE, one Block piece by piece in bounded memory: the Block decoder of common/block_decoder.c:64-200 for Blocks
+ * whose Compressed / Uncompressed Size is missing from the header (single-threaded encoders) or too large for a
+ * whole-Block job (4 GiB and more); the body of the direct mode of common/stream_decoder_mt.c.  LZMA2 alone: a
+ * Delta / BCJ chain gives XZB_OPTIONS_ERROR.
+ *   create  `header` is the whole Block Header (header_size bytes, as its first byte says), `check` the Stream's Check
+ *           ID, flags XZB_DEC_*.
+ *   code    takes the whole LZMA2 chunks at the front of in[0 .. in_size) (*in_used stops before a chunk that is not
+ *           all there; with finish != 0 that chunk is decoded as far as it goes and the Block ends in XZB_BUF_ERROR, as
+ *           input that ended early does), then the end marker, Block Padding and Check field, and returns 1
+ *           (LZMA_STREAM_END) once every byte of the Block is handed out.  Output that does not fit out_cap (any value,
+ *           0 included) stays on the GPU and is handed out first by the next call.  XZB_OK: call again with more input
+ *           or more room.  Verdicts are those of the Stream decoders (sizes against the header, Block Padding, Check
+ *           field unless XZB_DEC_IGNORE_CHECK), and the bytes decoded before an error are handed out before it.
+ *           Memory: the window holds up to twice the dictionary plus one piece (at most 64 MiB of output) on the GPU;
+ *           a dictionary so large that history and piece do not fit 32-bit window positions (dictionary property 40,
+ *           4 GiB - 1, once that much output exists) gives XZB_MEM_ERROR.
+ *   record  the Block's Index record, once code returned 1 (XZB_PROG_ERROR before).
+ */
+typedef struct xzb_block_decoder xzb_block_decoder;
+typedef struct {
+	uint64_t pieces, in_bytes, out_bytes;   /* pieces decoded, compressed bytes they took, bytes handed out */
+	uint64_t slides, bytes_slid;            /* moves of the history to the front of the window */
+	uint64_t window_bytes, max_history;     /* the window's size on the GPU, the largest history moved */
+	double ms_decode, ms_check, ms_d2h;     /* device time of the decode kernel, the check kernels, the output copies */
+} xzb_block_decoder_counters;
+int xzb_block_decoder_create(xzb_ctx *ctx, const uint8_t *header, uint32_t header_size, uint32_t check, uint32_t flags,
+		xzb_block_decoder **out);
+int xzb_block_decoder_code(xzb_block_decoder *bd, const uint8_t *in, uint64_t in_size, uint64_t *in_used,
+		uint8_t *out, uint64_t out_cap, uint64_t *out_size, uint32_t finish);
+int xzb_block_decoder_record(const xzb_block_decoder *bd, xzb_index_record *rec);
+int xzb_block_decoder_stats(const xzb_block_decoder *bd, xzb_block_decoder_counters *out);
+void xzb_block_decoder_destroy(xzb_block_decoder *bd);
+
 /* Device memory helpers for callers without a CUDA runtime binding (tests, bench). */
 int xzb_device_alloc(xzb_ctx *ctx, void **ptr, uint64_t size);
 void xzb_device_free(xzb_ctx *ctx, void *ptr);

@@ -38,6 +38,15 @@ class Stats(C.Structure):
         return {n: getattr(self, n) for n, _ in self._fields_}
 
 
+class BlockDecoderStats(C.Structure):
+    """xzb_block_decoder_counters: pieces, bytes, window slides, device times of one resumable Block decoder."""
+    _fields_ = [(n, C.c_uint64) for n in ("pieces", "in_bytes", "out_bytes", "slides", "bytes_slid", "window_bytes", "max_history")] + \
+               [(n, C.c_double) for n in ("ms_decode", "ms_check", "ms_d2h")]
+
+    def as_dict(self):
+        return {n: getattr(self, n) for n, _ in self._fields_}
+
+
 class XzError(RuntimeError):
     def __init__(self, code, msg=""):
         super().__init__(f"lzma_ret {code}: {msg}")
@@ -95,6 +104,11 @@ def lib():
         L.xzb_device_free.argtypes = [C.c_void_p, C.c_void_p]
         L.xzb_memcpy_h2d.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64]
         L.xzb_memcpy_d2h.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64]
+        L.xzb_block_decoder_create.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.POINTER(C.c_void_p)]
+        L.xzb_block_decoder_code.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, P64, C.c_void_p, C.c_uint64, P64, C.c_uint32]
+        L.xzb_block_decoder_record.argtypes = [C.c_void_p, C.POINTER(IndexRecord)]
+        L.xzb_block_decoder_stats.argtypes = [C.c_void_p, C.POINTER(BlockDecoderStats)]
+        L.xzb_block_decoder_destroy.argtypes = [C.c_void_p]
         _lib = L
     return _lib
 
@@ -196,6 +210,12 @@ class Context:
         if r != LZMA_OK:
             raise XzError(r, self._err())
         return bytes(out[: sz.value])
+
+    # ---- one Block piece by piece in bounded memory (xzb_block_decoder_*) ----
+    def block_decoder(self, header, check, flags=0):
+        """A resumable decoder of one LZMA2 Block whose whole Block Header is `header` in a Stream with Check ID `check`;
+        see BlockDecoder."""
+        return BlockDecoder(self, header, check, flags)
 
     # ---- lzma_stream_buffer_decode (one Stream): returns (ret, bytes, input bytes used) ----
     def stream_buffer_decode(self, data, cap, flags=0):
@@ -388,6 +408,60 @@ class Context:
         r = lib().xzb_memcpy_d2h(self._h, dp, d_src, n)
         if r != LZMA_OK:
             raise XzError(r, self._err())
+
+
+class BlockDecoder:
+    """xzb_block_decoder: .code(data, out_cap, finish) takes the whole LZMA2 chunks at the front of `data` (all of it
+    when finish), then the Block Padding and Check field, and returns (ret, bytes, in_used): ret 0 = call again with
+    the rest of the input (data[in_used:] first) or more room, 1 = the Block ended and every byte was handed out, else
+    the lzma_ret of the error (the bytes decoded before it come first).  .record() is the Block's Index record
+    (unpadded size, uncompressed size) after ret 1."""
+
+    def __init__(self, ctx, header, check, flags=0):
+        self._ctx = ctx
+        self._h = C.c_void_p()
+        hp, _k = _ptr(bytes(header))
+        r = lib().xzb_block_decoder_create(ctx._h, hp, len(header), check, flags, C.byref(self._h))
+        if r != LZMA_OK:
+            raise XzError(r, ctx._err())
+
+    def code(self, data, out_cap, finish=False):
+        out = (C.c_uint8 * max(out_cap, 1))()
+        dp, _k = _ptr(bytes(data) if data else b"\0")
+        used, size = C.c_uint64(), C.c_uint64()
+        r = lib().xzb_block_decoder_code(self._h, dp, len(data), C.byref(used), out, out_cap, C.byref(size), 1 if finish else 0)
+        return r, bytes(out[: size.value]), used.value
+
+    def code_into(self, src, n, dst, cap, finish=False):
+        """The same on caller-owned buffers (addresses or objects _ptr takes): (ret, bytes written, in_used)."""
+        sp, _k1 = _ptr(src)
+        dp, _k2 = _ptr(dst)
+        used, size = C.c_uint64(), C.c_uint64()
+        r = lib().xzb_block_decoder_code(self._h, sp, n, C.byref(used), dp, cap, C.byref(size), 1 if finish else 0)
+        return r, size.value, used.value
+
+    def record(self):
+        rec = IndexRecord()
+        r = lib().xzb_block_decoder_record(self._h, C.byref(rec))
+        if r != LZMA_OK:
+            raise XzError(r, "the Block has not ended")
+        return rec.unpadded_size, rec.uncompressed_size
+
+    def stats(self):
+        s = BlockDecoderStats()
+        lib().xzb_block_decoder_stats(self._h, C.byref(s))
+        return s
+
+    def close(self):
+        if self._h:
+            lib().xzb_block_decoder_destroy(self._h)
+            self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
 
 
 def index_encode(records):

@@ -154,7 +154,7 @@ XZB_HD_NOINLINE int xzb_lzma_chunk_decode(XzbDec *d, uint8_t *out, uint32_t *pos
 	}
 	rc.err = 0;
 	uint32_t state = d->state, rep0 = d->rep0, rep1 = d->rep1, rep2 = d->rep2, rep3 = d->rep3;
-	uint32_t prev = pos > dict_start ? out[pos - 1] : 0;  // previous byte, carried in a register
+	uint32_t prev = pos != dict_start ? out[pos - 1] : 0;  // previous byte, carried in a register (none right after a reset)
 	while (pos < limit && !rc.err) {
 		const uint32_t rel = pos - dict_start;  // dict.pos modulo 16 == bytes since dictionary reset modulo 16
 		const uint32_t pos_state = rel & d->pos_mask;
@@ -274,16 +274,37 @@ __device__ int xzb_lzma_chunk_decode_w(XzbDec *d, uint8_t *out, uint32_t *pos_pt
 		const uint32_t lane, XzbRcd *rcp);
 #endif
 
-// lzma2_decode, lzma/lzma2_decoder.c:55-230.  Returns XZB_OK at the end marker,
-// XZB_DATA_ERROR, XZB_NEED_INPUT or XZB_NEED_OUTPUT.
-XZB_HD_NOINLINE int xzb_lzma2_decode(XzbDec *d, const uint8_t *in, uint32_t in_size, uint32_t dict_size,
-		uint8_t *out, uint32_t out_limit, uint32_t *in_used, uint32_t *out_used, uint32_t lane, uint32_t nlanes)
+// The dictionary size the LZ layer rounds to (lz_decoder.c:247-256).
+XZB_HD uint32_t xzb_dict_size_r(uint32_t dict_size)
 {
-	uint32_t dict_size_r = dict_size < 4096 ? 4096 : dict_size;  // lz_decoder.c:247-256
-	dict_size_r = dict_size_r > 0xFFFFFFF0u ? 0xFFFFFFF0u : (dict_size_r + 15) & ~15u;
-	uint32_t in_pos = 0, pos = 0, dict_start = 0;
-	bool need_properties = true, need_dictionary_reset = true;
-	uint32_t lc = 0, lp = 0, pb = 0;
+	const uint32_t r = dict_size < 4096 ? 4096 : dict_size;
+	return r > 0xFFFFFFF0u ? 0xFFFFFFF0u : (r + 15) & ~15u;
+}
+
+// The chunk walk's state between two chunks (lzma2_decoder.c:23-52): what a resumed walk carries over.  dict_start is
+// where the dictionary was last reset, in out[] positions; a resumed walk passes a virtual one (xzb_dec_resume.cuh).
+struct XzbWalk {
+	uint32_t need_properties, need_dictionary_reset;
+	uint32_t lc, lp, pb;
+	uint32_t dict_start;
+	uint32_t dict_reset;   // set when a chunk reset the dictionary in this call
+};
+XZB_HD void xzb_walk_init(XzbWalk *w)
+{
+	w->need_properties = 1; w->need_dictionary_reset = 1;
+	w->lc = w->lp = w->pb = 0; w->dict_start = 0; w->dict_reset = 0;
+}
+
+// lzma2_decode, lzma/lzma2_decoder.c:55-230, over whole or cut chunks from in[0 .. in_size), writing out[pos0 ..
+// out_limit).  Returns XZB_OK at the end marker, XZB_DATA_ERROR, XZB_NEED_INPUT or XZB_NEED_OUTPUT; the walk state
+// *w is read on entry and written back on return.  (Inlined into its two callers below, so that the whole-Block decode
+// keeps the walk state in registers as a plain local.)
+XZB_HD int xzb_lzma2_walk_body(XzbDec *d, XzbWalk *w, const uint8_t *in, uint32_t in_size, uint32_t dict_size_r,
+		uint8_t *out, uint32_t pos0, uint32_t out_limit, uint32_t *in_used, uint32_t *out_used, uint32_t lane, uint32_t nlanes)
+{
+	uint32_t in_pos = 0, pos = pos0, dict_start = w->dict_start;
+	bool need_properties = w->need_properties != 0, need_dictionary_reset = w->need_dictionary_reset != 0;
+	uint32_t lc = w->lc, lp = w->lp, pb = w->pb;
 	int ret;
 	for (;;) {
 		if (in_pos >= in_size) { ret = XZB_NEED_INPUT; break; }
@@ -298,7 +319,7 @@ XZB_HD_NOINLINE int xzb_lzma2_decode(XzbDec *d, const uint8_t *in, uint32_t in_s
 			else if (need_properties) { ret = XZB_DATA_ERROR; break; }
 			else if (control >= 0xA0) state_reset = true;
 		} else if (control > 2) { ret = XZB_DATA_ERROR; break; }
-		if (need_dictionary_reset) { need_dictionary_reset = false; dict_start = pos; }
+		if (need_dictionary_reset) { need_dictionary_reset = false; dict_start = pos; w->dict_reset = 1; }
 		uint32_t usize = 0;
 		if (is_lzma) {
 			if (in_size - in_pos < 2) { in_pos = in_size; ret = XZB_NEED_INPUT; break; }
@@ -347,6 +368,24 @@ XZB_HD_NOINLINE int xzb_lzma2_decode(XzbDec *d, const uint8_t *in, uint32_t in_s
 		if (ret != XZB_OK) break;
 		if (in_pos - chunk_start != csize) { ret = XZB_DATA_ERROR; break; }  // :190-193
 	}
-	*in_used = in_pos; *out_used = pos;
+	w->need_properties = need_properties; w->need_dictionary_reset = need_dictionary_reset;
+	w->lc = lc; w->lp = lp; w->pb = pb; w->dict_start = dict_start;
+	*in_used = in_pos; *out_used = pos - pos0;
 	return ret;
+}
+
+// A run of chunks of a Block decoded piece by piece (xzb_dec_resume.cuh).
+XZB_HD_NOINLINE int xzb_lzma2_walk(XzbDec *d, XzbWalk *w, const uint8_t *in, uint32_t in_size, uint32_t dict_size_r,
+		uint8_t *out, uint32_t pos0, uint32_t out_limit, uint32_t *in_used, uint32_t *out_used, uint32_t lane, uint32_t nlanes)
+{
+	return xzb_lzma2_walk_body(d, w, in, in_size, dict_size_r, out, pos0, out_limit, in_used, out_used, lane, nlanes);
+}
+
+// One whole Block's LZMA2 data into out[0 .. out_limit).
+XZB_HD_NOINLINE int xzb_lzma2_decode(XzbDec *d, const uint8_t *in, uint32_t in_size, uint32_t dict_size,
+		uint8_t *out, uint32_t out_limit, uint32_t *in_used, uint32_t *out_used, uint32_t lane, uint32_t nlanes)
+{
+	XzbWalk w;
+	xzb_walk_init(&w);
+	return xzb_lzma2_walk_body(d, &w, in, in_size, xzb_dict_size_r(dict_size), out, 0, out_limit, in_used, out_used, lane, nlanes);
 }

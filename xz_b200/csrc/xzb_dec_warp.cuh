@@ -82,7 +82,7 @@ __device__ __noinline__ int xzb_lzma_chunk_decode_w(XzbDec *d, uint8_t *out, uin
 	rc.nb = rc.cur < rc.end ? (uint32_t)*rc.cur : 0u;
 	uint32_t derr = 0;   // XZB_DATA_ERROR found by the LZ layer
 	uint32_t state = d->state, rep0 = d->rep0, rep1 = d->rep1, rep2 = d->rep2, rep3 = d->rep3;
-	uint32_t prev = pos > dict_start ? out[pos - 1] : 0;   // previous byte when prev_ok
+	uint32_t prev = pos != dict_start ? out[pos - 1] : 0;  // previous byte when prev_ok (none right after a reset)
 	bool prev_ok = true;
 	uint32_t pend_pos = 0, pend_len = 0, pend_val = 0;     // bytes out[pend_pos + lane], lane < pend_len, loaded but not stored yet
 	while (pos < limit && !rc.err && !derr) {

@@ -20,6 +20,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <new>
 #include <vector>
 
 #include "../../include/xzb200.h"
@@ -30,6 +31,7 @@
 #include "xzb_sha256.cuh"
 #include "xzb_frame.cuh"
 #include "xzb_dec_stream.cuh"
+#include "xzb_dec_resume.cuh"
 #include "xzb_filters.cuh"
 #include "xzb_params.h"
 #include "xzb_parse_warp.cuh"
@@ -544,6 +546,78 @@ xzb_k_decode(const XzbDecJob *__restrict__ jobs, XzbDecResult *__restrict__ resu
 	if (threadIdx.x == 0) { results[b].ret = (uint32_t)ret; results[b].in_used = iu; results[b].out_used = ou; }
 }
 
+// ---- resumable Block decode (xzb_block_decoder_*, xzb_dec_resume.cuh) ----
+// The per-job state record in HBM: the probability model and the walk / position state between two pieces.
+struct XzbResumeRec {
+	XzbDec model;
+	XzbResume r;
+};
+struct XzbResJob {
+	const uint8_t *in;
+	uint32_t in_size;
+	uint32_t pos, out_limit;    // the piece writes win[pos .. out_limit)
+	uint8_t *win;
+	XzbResumeRec *rec;
+};
+
+// One warp per job, as xzb_k_decode: the model comes from the job's record into shared memory (not when the piece's first
+// chunk resets it anyway), the piece's chunks are decoded by the same walk and chunk decoder, and the model and state go
+// back to the record.
+__global__ void __launch_bounds__(32)
+xzb_k_decode_resume(const XzbResJob *__restrict__ jobs, XzbDecResult *__restrict__ results)
+{
+	extern __shared__ __align__(16) uint8_t xzb_smem[];
+	XzbDec *d = reinterpret_cast<XzbDec *>(xzb_smem);
+	const XzbResJob job = jobs[blockIdx.x];
+	XzbResume r = job.rec->r;
+	// The model is not loaded when the piece's first chunk must reset it: a control byte >= 0xA0 resets state (and 0xC0+
+	// the properties), and with need_properties set every LZMA chunk either resets it or is an error.  Whatever the
+	// shared memory held is then either overwritten before use or belongs to a Block that has failed (every error ends
+	// the Block), so storing it back is harmless.  tests/hostsim/block_dec_host.cpp garbles its model in the same case.
+	const bool fresh = job.in_size != 0 && (job.in[0] >= 0xA0 || r.walk.need_properties);
+	uint32_t *sm = reinterpret_cast<uint32_t *>(d);
+	uint32_t *gm = reinterpret_cast<uint32_t *>(&job.rec->model);
+	const uint32_t words = sizeof(XzbDec) / 4;
+	if (!fresh) for (uint32_t i = threadIdx.x; i < words; i += 32) sm[i] = gm[i];
+	__syncwarp();
+	uint32_t iu = 0, ou = 0;
+	const int ret = xzb_resume_piece(d, &r, job.in, job.in_size, job.win, job.pos, job.out_limit, &iu, &ou, threadIdx.x, 32);
+	__syncwarp();
+	for (uint32_t i = threadIdx.x; i < words; i += 32) gm[i] = sm[i];
+	if (threadIdx.x == 0) {
+		job.rec->r = r;
+		results[blockIdx.x].ret = (uint32_t)ret; results[blockIdx.x].in_used = iu; results[blockIdx.x].out_used = ou;
+	}
+}
+
+// memmove(dst, src, n) for dst < src with overlapping ranges: one CTA walks the range front to back in tiles that are
+// read whole before any of their bytes is written; a tile's destination lies below its source, and every later tile's
+// source lies above every earlier tile's destination.
+__global__ void __launch_bounds__(1024)
+xzb_k_move_down(uint8_t *dst, const uint8_t *src, uint32_t n)
+{
+	const uint32_t T = 1024, per = 16, tile = T * per;
+	for (uint32_t base = 0; base < n; base += tile) {
+		uint8_t v[per];
+#pragma unroll
+		for (uint32_t k = 0; k < per; ++k) { const uint32_t i = base + k * T + threadIdx.x; v[k] = i < n ? src[i] : 0; }
+		__syncthreads();
+#pragma unroll
+		for (uint32_t k = 0; k < per; ++k) { const uint32_t i = base + k * T + threadIdx.x; if (i < n) dst[i] = v[k]; }
+		__syncthreads();
+	}
+}
+
+// SHA-256 of a message that arrives in pieces: thread 0 feeds data[0 .. size) to the state record.
+__global__ void __launch_bounds__(32)
+xzb_k_sha256_update(XzbSha256State *st, const uint8_t *__restrict__ data, uint32_t size)
+{
+	if (threadIdx.x != 0) return;
+	XzbSha256State s = *st;
+	xzb_sha256_update(&s, data, size);
+	*st = s;
+}
+
 // ---- device-resident Stream decode (xzb_stream_buffer_decode_batch_device) ----
 // Each round: xzb_k_dec_scan (the next run of every unfinished item, xzb_dec_scan) -> xzb_k_decode over the run's
 // Blocks -> xzb_k_dec_prep (filter and check job lists) -> xzb_k_filter per chain level -> xzb_k_crc / xzb_k_sha256
@@ -791,6 +865,7 @@ extern "C" int xzb_ctx_create(xzb_ctx **out, int device)
 		const char *mw = getenv("XZB_MAX_WAVE_BLOCKS");
 		ctx->max_wave_blocks = mw ? (uint32_t)atoi(mw) : 0;
 		cudaFuncSetAttribute(xzb_k_decode, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(XzbDec));
+		cudaFuncSetAttribute(xzb_k_decode_resume, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(XzbDec));
 		if (cudaFuncSetAttribute(xzb_k_parse_dp, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(DS)) != cudaSuccess
 				|| cudaFuncSetAttribute(xzb_k_parse_fast<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)XZB_SOLO_SMEM) != cudaSuccess) {
 			fprintf(stderr, "xzb200: cannot reserve %zu B of shared memory for the parser kernel\n", sizeof(DS));
@@ -2075,6 +2150,181 @@ extern "C" int xzb_stream_buffer_decode_batch_device(xzb_ctx *ctx, uint32_t n, c
 	ctx->stats.ms_total = ev_ms(ctx->ev[6], ctx->ev[7]);
 	ctx->stats.ms_other = std::max(0.0, ctx->stats.ms_total - ctx->stats.ms_decode);
 	return XZB_OK;
+}
+
+// ------------------------------------------------------------------------------------
+// Resumable Block decoder (xzb_block_decoder_*): XzbBlockDec (xzb_dec_resume.cuh) over device memory
+// ------------------------------------------------------------------------------------
+// The window and the state record live in HBM; a piece's compressed bytes go up, its output comes down when the caller
+// takes it.  Every step ends in a synchronise: the next step's plan depends on the piece's results.
+struct XzbGpuBlockBackend {
+	xzb_ctx *ctx = nullptr;
+	uint8_t *win = nullptr;
+	uint8_t *in = nullptr; uint64_t in_cap = 0;
+	XzbResumeRec *rec = nullptr;
+	uint8_t *small = nullptr;   // job, result, check job, check value, SHA-256 state
+	xzb_block_decoder_counters st;
+	static const size_t OFF_JOB = 0, OFF_RES = 64, OFF_CJOB = 128, OFF_CVAL = 192, OFF_SHA = 256, SMALL = 512;
+
+	int init(xzb_ctx *c)
+	{
+		ctx = c;
+		memset(&st, 0, sizeof(st));
+		CK(cudaMalloc(&rec, sizeof(XzbResumeRec)));
+		CK(cudaMalloc(&small, SMALL));
+		XzbSha256State s0; xzb_sha256_init(&s0);
+		CK(cudaMemcpy(small + OFF_SHA, &s0, sizeof(s0), cudaMemcpyHostToDevice));
+		return XZB_OK;
+	}
+	void release()
+	{
+		if (win) cudaFree(win);
+		if (in) cudaFree(in);
+		if (rec) cudaFree(rec);
+		if (small) cudaFree(small);
+		win = in = small = nullptr; rec = nullptr;
+	}
+	int put_state(const XzbResume &r) { CK(cudaMemcpy(&rec->r, &r, sizeof(r), cudaMemcpyHostToDevice)); return XZB_OK; }
+	int reserve(uint64_t cap, uint32_t keep)
+	{
+		uint8_t *w = nullptr;
+		CK(cudaMalloc(&w, cap));
+		if (keep) { const cudaError_t e = cudaMemcpyAsync(w, win, keep, cudaMemcpyDeviceToDevice, ctx->stream); if (e != cudaSuccess) { cudaFree(w); CK(e); } }
+		CK(cudaStreamSynchronize(ctx->stream));
+		if (win) cudaFree(win);
+		win = w;
+		st.window_bytes = cap;
+		return XZB_OK;
+	}
+	// dst < src: one copy when the ranges do not overlap (the slide rule of XzbBlockDec::make_room), else one launch of
+	// the front-to-back move kernel
+	int move(uint32_t dst, uint32_t src, uint32_t n)
+	{
+		if (src - dst >= n) CK(cudaMemcpyAsync(win + dst, win + src, n, cudaMemcpyDeviceToDevice, ctx->stream));
+		else xzb_k_move_down<<<1, 1024, 0, ctx->stream>>>(win + dst, win + src, n);
+		CK(cudaStreamSynchronize(ctx->stream));
+		CK(cudaGetLastError());
+		st.slides += 1; st.bytes_slid += n;
+		return XZB_OK;
+	}
+	int decode(const uint8_t *src, uint32_t in_size, uint32_t pos, uint32_t out_limit, XzbResume *r, uint32_t *iu, uint32_t *ou, int *ret)
+	{
+		cudaStream_t s = ctx->stream;
+		if (in_cap < (uint64_t)in_size + 64) {
+			if (in) cudaFree(in);
+			in = nullptr; in_cap = 0;
+			const uint64_t want = std::max<uint64_t>((uint64_t)in_size + 64, 1u << 20);
+			CK(cudaMalloc(&in, want));
+			in_cap = want;
+		}
+		XzbResJob job{ in, in_size, pos, out_limit, win, rec };
+		CK(cudaMemcpyAsync(in, src, in_size, cudaMemcpyHostToDevice, s));
+		CK(cudaMemcpyAsync(small + OFF_JOB, &job, sizeof(job), cudaMemcpyHostToDevice, s));
+		CK(cudaEventRecord(ctx->ev[0], s));
+		xzb_k_decode_resume<<<1, 32, sizeof(XzbDec), s>>>((const XzbResJob *)(small + OFF_JOB), (XzbDecResult *)(small + OFF_RES));
+		CK(cudaEventRecord(ctx->ev[1], s));
+		XzbDecResult res;
+		CK(cudaMemcpyAsync(&res, small + OFF_RES, sizeof(res), cudaMemcpyDeviceToHost, s));
+		CK(cudaMemcpyAsync(r, &rec->r, sizeof(XzbResume), cudaMemcpyDeviceToHost, s));
+		CK(cudaStreamSynchronize(s));
+		CK(cudaGetLastError());
+		st.pieces += 1; st.in_bytes += in_size;
+		st.ms_decode += ev_ms(ctx->ev[0], ctx->ev[1]);
+		*iu = res.in_used; *ou = res.out_used; *ret = (int)res.ret;
+		return XZB_OK;
+	}
+	int check(uint32_t id, uint32_t pos, uint32_t n, uint64_t *crc)
+	{
+		cudaStream_t s = ctx->stream;
+		CK(cudaEventRecord(ctx->ev[2], s));
+		if (id == 10) {
+			xzb_k_sha256_update<<<1, 32, 0, s>>>((XzbSha256State *)(small + OFF_SHA), win + pos, n);
+		} else {
+			const XzbCrcJob cj{ win + pos, n };
+			CK(cudaMemcpyAsync(small + OFF_CJOB, &cj, sizeof(cj), cudaMemcpyHostToDevice, s));
+			const bool c64 = id == 4;
+			xzb_k_crc<<<1, 1024, 0, s>>>((const XzbCrcJob *)(small + OFF_CJOB), c64 ? ctx->d_crc64 : ctx->d_crc32w, c64 ? ~0ull : 0xFFFFFFFFull,
+					(uint64_t *)(small + OFF_CVAL), 1, nullptr);
+			CK(cudaMemcpyAsync(crc, small + OFF_CVAL, 8, cudaMemcpyDeviceToHost, s));
+		}
+		CK(cudaEventRecord(ctx->ev[3], s));
+		CK(cudaStreamSynchronize(s));
+		CK(cudaGetLastError());
+		st.ms_check += ev_ms(ctx->ev[2], ctx->ev[3]);
+		return XZB_OK;
+	}
+	int sha_final(uint8_t out[32])
+	{
+		XzbSha256State h;
+		CK(cudaMemcpy(&h, small + OFF_SHA, sizeof(h), cudaMemcpyDeviceToHost));
+		xzb_sha256_final(&h, out);
+		return XZB_OK;
+	}
+	int fetch(uint8_t *dst, uint32_t pos, uint64_t n)
+	{
+		CK(cudaEventRecord(ctx->ev[4], ctx->stream));
+		CK(cudaMemcpyAsync(dst, win + pos, n, cudaMemcpyDeviceToHost, ctx->stream));
+		CK(cudaEventRecord(ctx->ev[5], ctx->stream));
+		CK(cudaStreamSynchronize(ctx->stream));
+		st.ms_d2h += ev_ms(ctx->ev[4], ctx->ev[5]);
+		st.out_bytes += n;
+		return XZB_OK;
+	}
+};
+
+struct xzb_block_decoder {
+	XzbBlockDec<XzbGpuBlockBackend> d;
+};
+
+extern "C" int xzb_block_decoder_create(xzb_ctx *ctx, const uint8_t *header, uint32_t header_size, uint32_t check, uint32_t flags,
+		xzb_block_decoder **out)
+{
+	*out = nullptr;
+	cudaSetDevice(ctx->device);
+	ctx->err[0] = 0;
+	if (check > 15) return set_err(ctx, XZB_PROG_ERROR, "check ID %u", check);
+	XzbBlockHeader hb;
+	const int r = xzb_block_header_decode(ctx->h_tab.crc32, header, header_size, &hb);
+	if (r != XZB_OK) return set_err(ctx, r == XZB_BUF_ERROR ? XZB_PROG_ERROR : r, "bad Block Header");
+	if (hb.hsize != header_size) return set_err(ctx, XZB_PROG_ERROR, "header_size %u, the header says %llu", header_size, (unsigned long long)hb.hsize);
+	if (hb.n_pre != 0) return set_err(ctx, XZB_OPTIONS_ERROR, "the resumable Block decoder takes LZMA2 alone (no Delta / BCJ)");
+	xzb_block_decoder *bd = new (std::nothrow) xzb_block_decoder();
+	if (bd == nullptr) return XZB_MEM_ERROR;
+	int e = bd->d.be.init(ctx);
+	if (e == XZB_OK) e = bd->d.init(ctx->h_tab.crc32, ctx->h_tab.crc64, hb, check, flags);
+	if (e == XZB_OK) e = bd->d.be.put_state(bd->d.r);
+	if (e != XZB_OK) { bd->d.be.release(); delete bd; return e; }
+	*out = bd;
+	return XZB_OK;
+}
+
+extern "C" int xzb_block_decoder_code(xzb_block_decoder *bd, const uint8_t *in, uint64_t in_size, uint64_t *in_used,
+		uint8_t *out, uint64_t out_cap, uint64_t *out_size, uint32_t finish)
+{
+	cudaSetDevice(bd->d.be.ctx->device);
+	return bd->d.code(in, in_size, in_used, out, out_cap, out_size, finish != 0);
+}
+
+extern "C" int xzb_block_decoder_record(const xzb_block_decoder *bd, xzb_index_record *rec)
+{
+	bd->d.record(rec);
+	return bd->d.phase == 2 && bd->d.ret == XZB_OK ? XZB_OK : XZB_PROG_ERROR;
+}
+
+extern "C" int xzb_block_decoder_stats(const xzb_block_decoder *bd, xzb_block_decoder_counters *out)
+{
+	*out = bd->d.be.st;
+	out->max_history = bd->d.max_history;
+	return XZB_OK;
+}
+
+extern "C" void xzb_block_decoder_destroy(xzb_block_decoder *bd)
+{
+	if (bd == nullptr) return;
+	cudaSetDevice(bd->d.be.ctx->device);
+	cudaStreamSynchronize(bd->d.be.ctx->stream);
+	bd->d.be.release();
+	delete bd;
 }
 
 static_assert(sizeof(FS<false>) <= XZB_SOLO_SMEM && 2 * XZB_SOLO_SMEM > 228 * 1024 && XZB_SOLO_SMEM <= 227 * 1024,

@@ -14,6 +14,7 @@
 #include "../../include/xzb200.h"
 #include "../../include/xzb200_lzma.h"
 #include "xzb_params.h"
+#include "xzb_dec_resume.cuh"
 
 namespace {
 
@@ -22,6 +23,8 @@ enum { KIND_ENCODER, KIND_DECODER };
 
 const size_t WAVE_BLOCKS = 64;  // Blocks encoded per GPU batch while streaming
 const size_t PART_BLOCKS = 64;  // complete Blocks decoded as a part while the rest of the Stream still arrives
+const size_t PIECE_IN = 1u << 20;      // buffered compressed bytes that start a piece of a Block decoded piece by piece
+const size_t BD_OUT_STEP = 8u << 20;   // output taken from the piece-by-piece Block decoder per call
 
 }  // namespace
 
@@ -82,7 +85,12 @@ struct GpuCoder {
 	std::vector<xzb_index_record> prior;  // records of the current Stream's Blocks that were already decoded and cut out of inbuf
 	lzma_ret dec_ret;
 	lzma_ret deferred;    // encoder: an option error the reference only reports from lzma_code (BCJ start-offset alignment)
-	size_t last_try;      // buffered size at the last speculative decode of a Stream with unsized Blocks (LZMA_RUN)
+	size_t last_try;      // buffered size at the last speculative decode of a Stream with unsized Delta / BCJ Blocks (LZMA_RUN)
+	// the Block being decoded piece by piece (xzb_block_decoder): its header and the input it consumed are cut out of
+	// inbuf, so its next bytes are at inbuf[dec_off + 12]
+	xzb_block_decoder *bd;
+	bool bd_end;          // its end marker is buffered: decode without waiting for PIECE_IN bytes
+	bool bd_more;         // it holds decoded bytes that did not fit the last call's output
 };
 
 namespace {
@@ -120,6 +128,7 @@ void internal_destroy(lzma_stream *strm)   // lzma_end, common.c:379-389
 void gpu_coder_end(void *coder, const lzma_allocator *allocator)
 {
 	GpuCoder *in = static_cast<GpuCoder *>(coder);
+	if (in->bd) xzb_block_decoder_destroy(in->bd);
 	for (xzb_ctx *c : in->pool) if (c) xzb_ctx_destroy(c);
 	in->~GpuCoder();
 	xfree(allocator, in);
@@ -186,6 +195,7 @@ lzma_ret internal_create(lzma_stream *strm, int kind, uintptr_t init_marker)
 	in->dec_ret = LZMA_OK;
 	in->deferred = LZMA_OK;
 	in->last_try = 0;
+	in->bd = nullptr; in->bd_end = in->bd_more = false;
 	// Devices: XZB_DEVICE=n pins everything to one GPU; otherwise the decoder uses device 0 and the threaded encoder deals
 	// the Blocks of a wave over all GPUs of the process (XZB_DEVICES=a,b,c restricts the set) -- the worker fan-out of
 	// stream_encoder_mt.c:362-595 / :716-888 behind the one lzma_stream_encoder_mt call.
@@ -357,6 +367,8 @@ const uint64_t MAX_RATIO = 8192;
 // First guess of a Stream's uncompressed size from its Block Headers.  Header fields come from untrusted input, so a
 // claimed size counts only as far as the compressed bytes can justify it; unsized Blocks start from a modest guess and
 // the caller grows the buffer when the decoder reports that the output did not fit.  Walks as stream_complete did.
+// (Unsized LZMA2-only Blocks never get here -- they are decoded piece by piece -- so the guess and the grow-and-retry
+// loop of decoder_code only serve unsized Blocks behind a Delta / BCJ chain.)
 uint64_t stream_out_bound(const std::vector<uint8_t> &b, size_t off, size_t len, bool complete)
 {
 	if (!complete) return (uint64_t)len * 16 + (1u << 20);
@@ -389,6 +401,7 @@ static size_t complete_blocks(const std::vector<uint8_t> &b, size_t *end, uint64
 		const uint64_t comp = f.comp.v, unc = f.uncomp.v;
 		if (f.comp.st == XZB_VLI_LONG || f.comp.end >= f.hsize || f.uncomp.st == XZB_VLI_LONG) break;
 		if (comp == 0 || comp > (1ull << 40) || unc > comp * MAX_RATIO + 65536) break;  // a size the payload cannot justify is left to the final pass
+		if (comp >= 0xFFFFFFF0ull || unc >= 0xFFFFFFF0ull) break;  // too large for a whole-Block job: decoded piece by piece
 		const uint64_t total = f.hsize + ((comp + 3) & ~3ull) + csize;
 		if (b.size() - ip < total) break;
 		ip += (size_t)total;
@@ -420,8 +433,66 @@ static bool footer_at_end(const std::vector<uint8_t> &b)
 	return xzb_stream_footer_decode(crc32_table(), b.data() + b.size() - 12, &check, &index_size) == XZB_OK;
 }
 
+// The Block at b[at], when this decoder takes it piece by piece: a complete, valid header of an LZMA2-only Block that
+// carries no Compressed / Uncompressed Size or one too large for a whole-Block job (xzb_dec_scan's 32-bit jobs).
+static bool resumable_at(const std::vector<uint8_t> &b, size_t at, XzbBlockHeader *hb)
+{
+	if (at >= b.size() || b[at] == 0x00) return false;
+	const size_t hs = ((size_t)b[at] + 1) * 4;
+	if (b.size() - at < hs || xzb_block_header_decode(crc32_table(), b.data() + at, hs, hb) != XZB_OK || hb->n_pre != 0) return false;
+	return hb->comp == UINT64_MAX || hb->uncomp == UINT64_MAX || hb->comp >= 0xFFFFFFF0ull || hb->uncomp >= 0xFFFFFFF0ull;
+}
+
+// Is the Block at b[at] one without sizes behind a Delta / BCJ chain?  Only those still go through the whole-Stream
+// decode whose end is guessed from a Stream Footer at the end of the buffer (under LZMA_RUN).
+static bool unsized_chain_at(const std::vector<uint8_t> &b, size_t at)
+{
+	XzbBlockHeader hb;
+	if (at >= b.size() || b[at] == 0x00) return false;
+	const size_t hs = ((size_t)b[at] + 1) * 4;
+	if (b.size() - at < hs || xzb_block_header_decode(crc32_table(), b.data() + at, hs, &hb) != XZB_OK) return false;
+	return hb.n_pre != 0 && (hb.comp == UINT64_MAX || hb.uncomp == UINT64_MAX);
+}
+
+// One step of the Block decoded piece by piece (block_decoder.c:64-200 through xzb_block_decoder): a piece is decoded
+// once PIECE_IN compressed bytes are buffered, the end marker is in, or at LZMA_FINISH, and only when outq is empty, so
+// host memory stays at one piece of input plus a partial chunk.  Returns false when lzma_code has to wait for input.
+static bool block_step(GpuCoder *in, lzma_action action)
+{
+	const size_t at = in->dec_off + 12;
+	const size_t avail = in->inbuf.size() - at;
+	const bool finish = action == LZMA_FINISH;
+	if (!in->bd_more && !in->bd_end && !finish && avail < PIECE_IN) {
+		XzbChunkRun run;
+		xzb_chunk_run(in->inbuf.data() + at, avail, UINT64_MAX, UINT64_MAX, &run);
+		if (!run.end) return false;
+		in->bd_end = true;
+	}
+	in->outq.resize(BD_OUT_STEP);   // (empty before: the caller's loop delivers first)
+	uint64_t used = 0, produced = 0;
+	const int r = xzb_block_decoder_code(in->bd, in->inbuf.data() + at, avail, &used, in->outq.data(), BD_OUT_STEP, &produced, finish);
+	in->outq.resize((size_t)produced);
+	in->progress_out += produced;
+	in->inbuf.erase(in->inbuf.begin() + at, in->inbuf.begin() + at + (size_t)used);
+	in->bd_more = r == 0 && produced == BD_OUT_STEP;
+	if (r == 0) return used != 0 || produced != 0;
+	if (r == 1) {   // LZMA_STREAM_END: the Block, its Padding and Check are in; its record waits for the real Index
+		xzb_index_record rec;
+		xzb_block_decoder_record(in->bd, &rec);
+		in->prior.push_back(rec);
+	} else {        // the bytes decoded before the error are in outq; "input ended early" latches as below
+		in->finished = true;
+		in->dec_ret = r == 10 ? LZMA_OK : (lzma_ret)r;
+	}
+	xzb_block_decoder_destroy(in->bd);
+	in->bd = nullptr; in->bd_end = in->bd_more = false;
+	return true;
+}
+
 // stream_decode, common/stream_decoder.c:101-378, as a resumable loop over the buffered input: a
 // Stream is decoded as one GPU batch as soon as it is completely buffered (or at LZMA_FINISH).
+// Blocks without sizes (and LZMA2 Blocks too large for a whole-Block job) are decoded piece by piece as their input
+// arrives (block_step), with output as they go.
 // LZMA_TELL_* codes are returned once per Stream right after its header (:139-151).  With
 // LZMA_CONCATENATED (:334-371) Stream Padding must be a multiple of four zero bytes and the
 // decoder only finishes at LZMA_FINISH.
@@ -459,33 +530,18 @@ lzma_ret decoder_code(GpuCoder *in, const uint8_t *src, size_t *in_pos, size_t i
 				if (in->flags & LZMA_TELL_ANY_CHECK) return LZMA_GET_CHECK;
 			}
 		}
+		if (in->bd != nullptr) {
+			if (block_step(in, action)) continue;
+			return LZMA_OK;
+		}
 		// the not yet decoded rest of the input as its own buffer for the bound helpers
 		std::vector<uint8_t> rest;
 		const std::vector<uint8_t> *view = &in->inbuf;
 		if (in->dec_off != 0) { rest.assign(in->inbuf.begin() + in->dec_off, in->inbuf.end()); view = &rest; }
-		size_t end = 0;
-		const bool complete = stream_complete(*view, &end);
-		bool speculative = false;
-		if (!complete && action != LZMA_FINISH) {
-			// Progressive output: once PART_BLOCKS complete Blocks are waiting they are decoded as a part (wrapped
-			// with an Index + Footer made from their own headers, so the one-shot decoder validates each Block
-			// exactly as it would inside the whole Stream) and cut out of the buffer; their records go to
-			// `prior` for the check of the real Index at the end.
-			size_t bend = 0; uint64_t unc = 0;
-			std::vector<xzb_index_record> recs(in->prior);
-			const size_t nb = complete_blocks(*view, &bend, &unc, &recs);
-			if (nb < PART_BLOCKS) {
-				// Unsized Blocks hide the end of the Stream; the reference's decoder returns LZMA_STREAM_END under LZMA_RUN
-				// once the footer is in (stream_decoder.c:309-331).  When the buffered bytes end in a valid Stream Footer
-				// the whole buffer is decoded; "input ended early" from that attempt just means: not yet.
-				if (view->size() != in->last_try && footer_at_end(*view)) {
-					in->last_try = view->size();
-					speculative = true;
-				} else {
-					return LZMA_OK;
-				}
-			}
-			if (!speculative) {
+		// A part of complete sized Blocks (wrapped with an Index + Footer made from their own headers, so the one-shot
+		// decoder validates each Block exactly as it would inside the whole Stream) is decoded and cut out of the buffer;
+		// its records go to `prior` for the check of the real Index at the end.  Returns -1 to go on, else lzma_code's code.
+		auto decode_part = [&](size_t bend, uint64_t unc, std::vector<xzb_index_record> &recs) -> int {
 			uint64_t mu = 0; uint32_t exceeds = 0;
 			xzb_stream_memusage(in->ctx, view->data(), bend, in->memlimit, &mu, &exceeds);
 			in->memusage = mu;
@@ -502,10 +558,52 @@ lzma_ret decoder_code(GpuCoder *in, const uint8_t *src, size_t *in_pos, size_t i
 					in->prior.data(), in->prior.size());
 			in->outq.resize(at + (size_t)produced);
 			in->progress_out += produced;
-			if (r != 0) { in->finished = true; in->dec_ret = (lzma_ret)r; continue; }
+			if (r != 0) { in->finished = true; in->dec_ret = (lzma_ret)r; return -1; }
 			in->prior.swap(recs);
 			in->inbuf.erase(in->inbuf.begin() + in->dec_off + 12, in->inbuf.begin() + in->dec_off + bend);
+			return -1;
+		};
+		size_t bend = 0; uint64_t unc = 0;
+		std::vector<xzb_index_record> recs(in->prior);
+		const size_t nb = complete_blocks(*view, &bend, &unc, &recs);
+		XzbBlockHeader nh;
+		// (a Stream Header that does not decode is left to the whole-Stream path below, which reports it before any Block)
+		if (header_check_id(view->data()) >= 0 && resumable_at(*view, bend, &nh)) {
+			// the complete sized Blocks in front of it first (a part of fewer than PART_BLOCKS), then the Block itself
+			if (nb > 0) {
+				const int rp = decode_part(bend, unc, recs);
+				if (rp >= 0) return (lzma_ret)rp;
+				continue;
+			}
+			// SEQ_BLOCK_INIT memory limit, stream_decoder.c:199-232 (recoverable: lzma_memlimit_set + lzma_code again)
+			in->memusage = (uint64_t)nh.dict_size + 66200;
+			if (in->memusage > in->memlimit) return LZMA_MEMLIMIT_ERROR;
+			const int r = xzb_block_decoder_create(in->ctx, view->data() + 12, (uint32_t)nh.hsize, in->cur_check, dec_flags(in->flags), &in->bd);
+			if (r != 0) { in->finished = true; in->dec_ret = (lzma_ret)r; continue; }
+			in->inbuf.erase(in->inbuf.begin() + in->dec_off + 12, in->inbuf.begin() + in->dec_off + 12 + (size_t)nh.hsize);
 			continue;
+		}
+		size_t end = 0;
+		const bool complete = stream_complete(*view, &end);
+		bool speculative = false;
+		if (!complete && action != LZMA_FINISH) {
+			// Progressive output: once PART_BLOCKS complete Blocks are waiting they are decoded as a part.
+			if (nb < PART_BLOCKS) {
+				// An unsized Block behind a Delta / BCJ chain (LZMA2-only ones went to block_step above) hides the end of
+				// the Stream; the reference's decoder returns LZMA_STREAM_END under LZMA_RUN once the footer is in
+				// (stream_decoder.c:309-331).  When the buffered bytes end in a valid Stream Footer the whole buffer is
+				// decoded; "input ended early" from that attempt just means: not yet.
+				if (view->size() != in->last_try && unsized_chain_at(*view, bend) && footer_at_end(*view)) {
+					in->last_try = view->size();
+					speculative = true;
+				} else {
+					return LZMA_OK;
+				}
+			}
+			if (!speculative) {
+				const int rp = decode_part(bend, unc, recs);
+				if (rp >= 0) return (lzma_ret)rp;
+				continue;
 			}
 		}
 		{  // SEQ_BLOCK_INIT memory limit, stream_decoder.c:199-232 (recoverable: lzma_memlimit_set + lzma_code again)

@@ -75,3 +75,52 @@ XZB_HD void xzb_sha256(const uint8_t *data, uint32_t size, uint8_t out[32])
 	}
 	for (int i = 0; i < 8; ++i) { out[4 * i] = (uint8_t)(h[i] >> 24); out[4 * i + 1] = (uint8_t)(h[i] >> 16); out[4 * i + 2] = (uint8_t)(h[i] >> 8); out[4 * i + 3] = (uint8_t)h[i]; }
 }
+
+// The same hash over a message that arrives in pieces (a Block decoded chunk run by chunk run): the chaining value,
+// the byte count and the partial 64-byte block live in a plain struct that can sit in device memory between calls.
+struct XzbSha256State {
+	uint32_t h[8];
+	uint64_t count;      // bytes hashed so far
+	uint8_t buf[64];     // the partial block: count % 64 bytes
+};
+XZB_HD void xzb_sha256_init(XzbSha256State *s)
+{
+	const uint32_t iv[8] = { 0x6a09e667u, 0xbb67ae85u, 0x3c6ef372u, 0xa54ff53au, 0x510e527fu, 0x9b05688cu, 0x1f83d9abu, 0x5be0cd19u };
+	for (int i = 0; i < 8; ++i) s->h[i] = iv[i];
+	s->count = 0;
+}
+XZB_HD void xzb_sha256_update(XzbSha256State *s, const uint8_t *data, uint64_t size)
+{
+	uint32_t w[16];
+	uint32_t have = (uint32_t)(s->count & 63);
+	s->count += size;
+	uint64_t pos = 0;
+	if (have) {
+		while (have < 64 && pos < size) s->buf[have++] = data[pos++];
+		if (have < 64) return;
+		for (int i = 0; i < 16; ++i) w[i] = xzb_be32(s->buf + 4 * i);
+		xzb_sha256_compress(s->h, w);
+	}
+	for (; size - pos >= 64; pos += 64) {
+		for (int i = 0; i < 16; ++i) w[i] = xzb_be32(data + pos + 4 * i);
+		xzb_sha256_compress(s->h, w);
+	}
+	for (uint32_t i = 0; pos < size; ++i) s->buf[i] = data[pos++];
+}
+XZB_HD void xzb_sha256_final(XzbSha256State *s, uint8_t out[32])
+{
+	uint32_t w[16];
+	uint8_t tail[128];
+	const uint32_t rem = (uint32_t)(s->count & 63);
+	for (uint32_t i = 0; i < rem; ++i) tail[i] = s->buf[i];
+	tail[rem] = 0x80;
+	const uint32_t total = rem + 1 + 8 <= 64 ? 64u : 128u;
+	for (uint32_t i = rem + 1; i < total - 8; ++i) tail[i] = 0;
+	const uint64_t bits = s->count * 8;
+	for (int i = 0; i < 8; ++i) tail[total - 1 - i] = (uint8_t)(bits >> (8 * i));
+	for (uint32_t c = 0; c < total; c += 64) {
+		for (int i = 0; i < 16; ++i) w[i] = xzb_be32(tail + c + 4 * i);
+		xzb_sha256_compress(s->h, w);
+	}
+	for (int i = 0; i < 8; ++i) { out[4 * i] = (uint8_t)(s->h[i] >> 24); out[4 * i + 1] = (uint8_t)(s->h[i] >> 16); out[4 * i + 2] = (uint8_t)(s->h[i] >> 8); out[4 * i + 3] = (uint8_t)s->h[i]; }
+}
