@@ -368,9 +368,9 @@ xzb_k_parse_dp(const XzbEncJob *__restrict__ jobs, const XzbMfBlock *__restrict_
 	}
 	if (threadIdx.x < 32) S.prep[threadIdx.x] = make_uint4(0u, 0u, 0u, 0u);
 	if (threadIdx.x <= DP_WMAX) S.idle[threadIdx.x] = 0;
-	if (threadIdx.x < 32) { S.part_tag[threadIdx.x] = 0; S.res_c[threadIdx.x] = make_uint4(0u, 0u, 0u, 0u); }
+	if (threadIdx.x < 32) { S.part_tag[threadIdx.x] = 0; S.res_c[threadIdx.x] = make_uint4(0u, 0u, 0u, 0u); S.lr[threadIdx.x] = make_uint2(0u, 0u); }
 #ifdef XZB_DP_PROF
-	if (threadIdx.x < 44) S.prof[threadIdx.x] = 0;
+	if (threadIdx.x < DP_NPROF) S.prof[threadIdx.x] = 0;
 #endif
 	for (uint32_t i = threadIdx.x; i < DP_NR; i += blockDim.x) S.ph[i] = 0;
 	__syncthreads();
@@ -416,6 +416,10 @@ xzb_k_parse_dp(const XzbEncJob *__restrict__ jobs, const XzbMfBlock *__restrict_
 			printf("DPPROF loop top + instrumentation: %.0f cyc/node; worker0 near path (node final seen -> near candidates pushed): %.0f cyc x %llu\n",
 				(double)S.prof[7] / ((double)S.prof[4] + 1e-9), (double)S.prof[29] / ((double)S.prof[30] + 1e-9), S.prof[30]);
 			printf("DPPROF gather: slots that had to wait for node t-2: %llu, t-3: %llu, t-4: %llu, t-5..8: %llu, older: %llu\n", S.prof[24], S.prof[25], S.prof[26], S.prof[27], S.prof[28]);
+			printf("DPPROF gather, last failed poll of a slot (t-2 / t-3 / t-4 / t-5..8 / older): phase flag %llu / %llu / %llu / %llu / %llu, \"literal + rep0\" %llu / %llu / %llu / %llu / %llu\n",
+				S.prof[44], S.prof[45], S.prof[46], S.prof[47], S.prof[48], S.prof[49], S.prof[50], S.prof[51], S.prof[52], S.prof[53]);
+			printf("DPPROF worker nodes: not rare %llu with the near wave + %llu without, rare %llu with + %llu without; \"literal + rep0\" onto c+3 %llu, possible %llu, applied %llu, of them extending the segment %llu\n",
+				S.prof[54], S.prof[55], S.prof[57], S.prof[58], S.prof[56], S.prof[59], S.prof[60], S.prof[61]);
 			const double ns = (double)S.prof[15] + 1e-9, ng = (double)S.prof[19] + 1e-9;
 			printf("DPPROF symbols %llu: optimum_normal %.0f cyc/symbol, encode_symbol %.0f cyc x %llu, chunk-loop tests %.0f cyc/iteration | segments %llu: helper1 %.0f idle_wait %.0f backward %.0f cyc/segment\n",
 				S.prof[15], S.prof[13] / ns, S.prof[14] / ((double)S.prof[43] + 1e-9), S.prof[43], S.prof[42] / ((double)S.prof[36] + S.prof[43] + 1e-9), S.prof[19], S.prof[16] / ng, S.prof[17] / ng, S.prof[18] / ng);

@@ -20,7 +20,8 @@
 //     compares for the four reps and pushes the node's candidates into ITS OWN ring of 16-byte
 //     slots (price, back, packed link incl. the target's match byte, back_2) -- private rings, so no
 //     atomics -- in three waves ordered by distance (targets <= +3, <= +8, rest), publishing a phase
-//     flag after each; the chain warp only waits for the wave it needs.
+//     flag after each; the chain warp only waits for the wave it needs.  "Literal + rep0" needs the
+//     chain's verdict on slot cur+1 and comes last; only the one slot it lands on waits for it.
 //   * Exactness of ties (strict '<' keeps the first candidate in the reference's program order,
 //     DESIGN.md F3): inside a ring candidates are applied class by class in program order; across
 //     rings the gather prefers the lower source node; the one candidate that must be applied late
@@ -42,11 +43,14 @@
 #define DP_T(v) const long long v = clock64()
 #define DP_ACC(i, a, b) do { if (blockIdx.x == 0) S.prof[i] += (unsigned long long)((b) - (a)); } while (0)
 #define DP_CNT(i) do { if (blockIdx.x == 0) S.prof[i] += 1; } while (0)
+#define DP_CNTA(i) do { if (blockIdx.x == 0) atomicAdd(&S.prof[i], 1ull); } while (0)   // from any worker warp
 #else
 #define DP_T(v)
 #define DP_ACC(i, a, b)
 #define DP_CNT(i)
+#define DP_CNTA(i)
 #endif
+#define DP_NPROF 62u
 
 // 16-byte shared-memory records are handed over with ONE vector store and polled with ONE vector load (an aligned
 // 16-byte access of one lane is a single shared-memory transaction, so the reader sees all of it or none)
@@ -61,6 +65,10 @@ __device__ __forceinline__ uint2 dp_lds64(const volatile void *p)
 	uint2 v;
 	asm volatile("ld.volatile.shared.v2.u32 {%0, %1}, [%2];" : "=r"(v.x), "=r"(v.y) : "r"((uint32_t)__cvta_generic_to_shared(const_cast<const void *>(p))) : "memory");
 	return v;
+}
+__device__ __forceinline__ void dp_sts64(volatile void *p, const uint2 v)
+{
+	asm volatile("st.volatile.shared.v2.u32 [%0], {%1, %2};" :: "r"((uint32_t)__cvta_generic_to_shared(const_cast<void *>(p))), "r"(v.x), "r"(v.y) : "memory");
 }
 __device__ __forceinline__ void dp_sts128(volatile void *p, const uint4 v)
 {
@@ -106,8 +114,7 @@ struct DS {  // dynamic shared memory of xzb_k_parse_dp
 	alignas(16) xzb_pair ring_mp[32][8];
 	uint32_t ring_mh[32];
 	uint32_t m_dist[XZB_MATCH_LEN_MAX + 1];
-	uint16_t m_len[XZB_MATCH_LEN_MAX + 1], m_len2[XZB_MATCH_LEN_MAX + 1];
-	uint8_t m_mb[XZB_MATCH_LEN_MAX + 1 + 2];
+	uint16_t m_len[XZB_MATCH_LEN_MAX + 1];
 	xzb_prob probs[PI_TOTAL + 2];
 	uint8_t prices[128];
 	alignas(8) uint16_t rc_bits[72];
@@ -136,8 +143,12 @@ struct DS {  // dynamic shared memory of xzb_k_parse_dp
 	volatile uint32_t rcq_T;                 // rc_out_pos + rc_cache_size at rcq_tail
 	volatile uint32_t rcq_flushes, rcq_out_pos;   // chunks finished, compressed size of the last one
 	volatile uint32_t part_tag[32];          // tagn(t) + 1
+	// owner worker -> gather / chain warp, per node c (ring c & 31): { tagn(c) + 1, the slot c's "literal + rep0" lands on
+	// while its push is pending, else 0 }; written before the node's first phase flag with ONE 8-byte store.  Only nodes
+	// t-2 .. t-W-1 are ever read, and node c-32's worker has finished it before slot c can finish, so 32 entries suffice.
+	alignas(8) uint2 lr[32];
 #ifdef XZB_DP_PROF
-	unsigned long long prof[44];
+	unsigned long long prof[DP_NPROF];
 #endif
 };
 
@@ -335,6 +346,11 @@ struct DpEnc : WarpEncT<DS> {
 		uint4 v = make_uint4(XZB_INFINITY_PRICE, 0, 0, 0);
 		uint4 *e = &S.ring_pool[(lane < W ? lane : 0) * rstride + (t & rmask)];
 		if (lane < W) { v = *e; e->x = XZB_INFINITY_PRICE; }   // the slot is free for node t + rsize
+		return best_of(t, v);
+	}
+	// the best of the lanes' ring entries for node t (lanes >= W hold none)
+	__device__ __forceinline__ uint4 best_of(uint32_t t, uint4 v)
+	{
 		const uint32_t m = __reduce_min_sync(WFULL, v.x);
 		const uint32_t src = (lane < W && v.x == m) ? DP_SRC(t, v.z) : DP_NONE;
 		const uint32_t s = __reduce_min_sync(WFULL, src);
@@ -348,23 +364,49 @@ struct DpEnc : WarpEncT<DS> {
 		const uint32_t v = S.ph[node & rmask];
 		return (v >> 2) == tagn(epoch, node) && (v & 3) >= need;
 	}
-	// Every candidate that can land on node t has been pushed: nodes t-2 .. t-W-1 are checked (node t-1 only reaches t
-	// through the chain warp's registers; anything older shares its worker with a checked node that has already started).
-	// Returns false when the segment was stopped meanwhile.
-	__device__ __forceinline__ bool wait_deadlines(uint32_t t)
+	// the slot node's "literal + rep0" is still to be pushed onto, else 0.  Loaded right behind the node's phase flag:
+	// loads are performed in order, so once the flag is seen the record is the one written before it (a node without a
+	// record -- fewer than 2 bytes left -- has no such candidate).
+	__device__ __forceinline__ uint32_t lr_target(uint32_t node) const
+	{
+		const uint2 r = dp_lds64(&S.lr[node & 31]);
+		return r.x == tagn(epoch, node) + 1 ? r.y : 0u;
+	}
+	// Every candidate that can land on node t has been pushed: nodes t-2 .. t-W-1 are checked -- the wave that covers t,
+	// and no "literal + rep0" pending onto t (node t-1 only reaches t through the chain warp's registers; anything older
+	// shares its worker with a checked node that has already started, and a worker finishes a node, "literal + rep0"
+	// included, before it starts the next).
+	// Lane d - 2 also loads slot t of ring wr, the ring of node t - d, with every poll, behind that node's flag and record:
+	// when the last flag is seen, v already is the final entry (no further round trip), and the slot is cleared for node
+	// t + rsize.  Returns false when the segment was stopped meanwhile.
+	__device__ __forceinline__ bool wait_deadlines(uint32_t t, uint32_t wr, uint4 &v)
 	{
 		const uint32_t d = lane + 2;
+		uint4 *const e = &S.ring_pool[(lane < W ? wr : 0) * rstride + (t & rmask)];
 		const bool mine = d <= W + 1 && t > d;   // node t - d >= 1
 		const uint32_t need = d <= 3 ? 1u : (d <= 8 ? 2u : 3u);
+#ifdef XZB_DP_PROF
+		const uint32_t dbin = d <= 4 ? d - 2 : d <= 8 ? 3 : 4;
+		uint32_t miss = 0;   // what this lane still waited for at the last failed poll: 1 = the phase flag, 2 = "literal + rep0"
+#endif
 		for (uint32_t it = 0;; ++it) {
-			const bool ok = !mine || ph_ok(t - d, need);
+			const bool okp = !mine || ph_ok(t - d, need);
+			const uint32_t lt = mine ? lr_target(t - d) : 0u;
+			if (lane < W) v = dp_lds128(e);
+			const bool ok = okp && lt != t;
 			if (__all_sync(WFULL, ok)) break;
 #ifdef XZB_DP_PROF
-			if (it == 0 && !ok && blockIdx.x == 0) atomicAdd((unsigned long long *)&S.prof[24 + (d <= 4 ? d - 2 : d <= 8 ? 3 : 4)], 1ull);   // which node the slot waits for
+			if (it == 0 && !ok && blockIdx.x == 0) atomicAdd(&S.prof[24 + dbin], 1ull);   // which node the slot waits for
+			miss = ok ? 0u : (okp ? 2u : 1u);
 #endif
 			if ((it & 15) == 15 && (S.seg_stop != DP_NONE || S.m_exit)) return false;
 		}
+#ifdef XZB_DP_PROF
+		if (miss != 0) DP_CNTA(44 + 5 * (miss - 1) + dbin);
+#endif
 		DP_ACQUIRE();
+		if (lane < W) e->x = XZB_INFINITY_PRICE;
+		else v = make_uint4(XZB_INFINITY_PRICE, 0, 0, 0);
 		return true;
 	}
 	__device__ __forceinline__ void wait_all_complete(uint32_t cur)   // nodes 1 .. cur-1 have pushed everything
@@ -372,7 +414,9 @@ struct DpEnc : WarpEncT<DS> {
 		const uint32_t d = lane + 1;
 		const bool mine = d <= W && cur > d;
 		for (;;) {
-			const bool ok = !mine || ph_ok(cur - d, 3);
+			const bool okp = !mine || ph_ok(cur - d, 3);
+			const uint32_t lt = mine ? lr_target(cur - d) : 0u;
+			const bool ok = okp && lt == 0;
 			if (__all_sync(WFULL, ok)) break;
 		}
 		DP_ACQUIRE();
@@ -857,10 +901,12 @@ __device__ inline void xzb_dp_gather_main(DS &S, DpEnc &H)
 		__threadfence_block();
 		my_epoch = e;
 		H.epoch = e;
-		for (uint32_t t = 2; t < XZB_OPTS; ++t) {
-			if (!H.wait_deadlines(t)) break;
+		uint32_t wr = lane < H.W ? H.W - 1 - lane : 0u;   // ring of node t - (lane + 2): worker (t - lane - 3) mod W
+		for (uint32_t t = 2; t < XZB_OPTS; ++t, wr = wr + 1 == H.W ? 0u : wr + 1) {
+			uint4 v;
+			if (!H.wait_deadlines(t, wr, v)) break;
 			// slot (t & 31) is free: the chain warp consumed node t - 32 long ago (it cannot be more than W + 1 nodes behind)
-			const uint4 v = H.gather(t);
+			v = H.best_of(t, v);
 			__syncwarp();
 			if (lane == 0) {
 				S.part[t & 31] = v;
@@ -1018,7 +1064,7 @@ __device__ inline void xzb_dp_worker_main(DS &S, DpEnc &H, const uint32_t w)
 			// =============== wait for the node itself ===============
 			const uint32_t k = c & rmask;
 			// Between here and the near-wave push nothing writes slots c + 2 and c + 3 of the own ring: this worker's earlier
-			// nodes are done, and the gather warp clears a slot only when it reads it, which waits for this node's wave 1.
+			// nodes are done ("literal + rep0" included), and the gather warp clears a slot only when it reads it, which waits for this node's wave 1.
 			// So the prices they hold now are the ones the push compares with, read off the path that follows the flag.
 			const uint32_t near_old = lane < 2 ? rg[(c + 2 + lane) & rmask].x : 0u;
 			DP_T(w0);
@@ -1039,6 +1085,7 @@ __device__ inline void xzb_dp_worker_main(DS &S, DpEnc &H, const uint32_t w)
 			const uint32_t hr[4] = { rr.x, rr.y, rr.z, rr.w };
 			const uint32_t baf = xzb_min(H.size - p, XZB_OPTS - 1 - c);   // buf_avail_full
 			const uint32_t nice_len = H.nice_len, pos_mask = H.pos_mask;
+			uint32_t lr_len = 0;   // "literal + rep0": len_test, 0 when there is no such candidate
 			if (baf >= 2) {
 				const uint32_t buf_avail = xzb_min(baf, nice_len);
 				const uint4 b0 = S.pb[st][ps][0], b1 = S.pb[st][ps][1];
@@ -1061,9 +1108,6 @@ __device__ inline void xzb_dp_worker_main(DS &S, DpEnc &H, const uint32_t w)
 				// of length 2 or 3 is a candidate follows from the compare mask alone: rep0 covers length L iff its first L
 				// bytes match, and a match candidate of length L exists iff rep0 does not cover L (start_len, :690-715).
 				bool near_done = false;
-				// "literal + rep0" of length exactly 2 lands on c + 3 (byte 0 differs, bytes 1-2 match, byte 3 does not):
-				// then wave 1 is complete only with it
-				const bool lr_near = (mg0 & 0xF) == 0x9;
 				{
 					const bool other_reps = ((rmaskb >> 8) & 3) == 0 || ((rmaskb >> 16) & 3) == 0 || ((rmaskb >> 24) & 3) == 0;
 					if (!other_reps && nice_len >= 8 && count <= 32) {
@@ -1078,13 +1122,26 @@ __device__ inline void xzb_dp_worker_main(DS &S, DpEnc &H, const uint32_t w)
 						if ((vr || vmn) && prn < near_old) rg[(c + L2) & rmask] = make_uint4(prn, bkn, men, 0u);   // H.push against near_old
 						__syncwarp();
 						near_done = true;
-						if (!lr_near) { DP_RELEASE(); if (lane == 0) S.ph[k] = (want << 2) | 1u; }
+						// "literal + rep0" of length exactly 2 (byte 0 differs, bytes 1-2 match, byte 3 does not) lands on c + 3:
+						// its record goes out with wave 1; any other target is announced below, before wave 2
+						if ((mg0 & 0xF) == 0x9 && lane == 0) dp_sts64(&S.lr[c & 31], make_uint2(want + 1, c + 3));
+						DP_RELEASE();
+						if (lane == 0) S.ph[k] = (want << 2) | 1u;
 						// len_end only has to grow before this node's last phase flag (the chain warp waits for every node to be
 						// complete before it ends the segment on len_end), so the atomic comes after the flag the gather waits for
 						if (lane == 0 && lb) atomicMax(&S.len_end_sh, c + lb);
 						{ DP_T(wn); if (lane == 0 && w == 0) { DP_ACC(29, w1, wn); DP_CNT(30); } }
 					}
 				}
+				// "literal + rep0" (:562-597) exists iff rep0 misses byte 0 and matches bytes 1 .. len_test, len_test >= 2; it
+				// lands on c + 1 + len_test.  Only whether it is pushed waits for the chain warp's verdict on slot c + 1, so
+				// its target is announced before the phase flag of the wave that covers it (the near wave's own record
+				// above) and the gather warp holds only that one slot for it.
+				if (mg0 & 1) {
+					const uint32_t lt = H.mlen_from(mg0, 1, buf_avail, b, bb0, xzb_min(baf, nice_len + 1)) - 1;
+					if (lt >= 2) lr_len = lt;
+				}
+				if (lane == 0) dp_sts64(&S.lr[c & 31], make_uint2(want + 1, lr_len ? c + 1 + lr_len : 0u));
 				uint32_t rlen[4];
 #pragma unroll
 				for (uint32_t ri = 0; ri < XZB_REPS; ++ri) {
@@ -1098,6 +1155,13 @@ __device__ inline void xzb_dp_worker_main(DS &S, DpEnc &H, const uint32_t w)
 				if (has_m) maxT = xzb_max(maxT, c + new_len);
 
 				if (lane == 0) atomicMax(&S.len_end_sh, maxT);
+#ifdef XZB_DP_PROF
+				if (lane == 0) {
+					DP_CNTA(rare ? (near_done ? 57 : 58) : (near_done ? 54 : 55));
+					if (lr_len == 2) DP_CNTA(56);   // lands on c + 3
+					if (lr_len != 0) DP_CNTA(59);
+				}
+#endif
 
 				// ---- this node's candidates, one lane each; the plain lengths first (the nearest targets are the urgent ones) ----
 				DpNodeCands K;
@@ -1186,55 +1250,13 @@ __device__ inline void xzb_dp_worker_main(DS &S, DpEnc &H, const uint32_t w)
 					H.push(rg, K.v_m && inL, c + Ln, K.pr_m, K.bk_m, K.me_m, 0);
 					__syncwarp();
 				};
-				// "literal + rep0" (:562-597) needs to know whether literal / short rep took slot c + 1
-				auto lit_rep0 = [&](const bool late) {
-					const uint32_t wantn = DpEnc::tagn(my_epoch, c);
-					uint32_t nv;
-					__syncwarp();
-					for (;;) {
-						nv = __shfl_sync(WFULL, S.nil_node, 0);
-						if ((nv >> 17) == (wantn >> 16) && ((nv >> 1) & 0xFFFF) >= c) break;
-						if (__shfl_sync(WFULL, (uint32_t)(S.seg_epoch != my_epoch || S.m_exit), 0)) return;
-					}
-					// the flag of node c itself; a later value means the chain warp is already past c + 1: read ours from the link
-					bool nil;
-					if (((nv >> 1) & 0xFFFF) == c) nil = (nv & 1) != 0;
-					else { DP_ACQUIRE(); const uint32_t m1 = S.o_meta[c + 1]; nil = DP_FLAGS(m1) == 0 && DP_D1(m1) == 1; }
-					if (nil || mb == cb) return;
-					DP_ACQUIRE();
-					const uint32_t c1 = S.n_c1[k];
-					const uint32_t limit = xzb_min(baf, nice_len + 1);
-					const uint32_t len_test = H.mlen_from(rmaskb & 0xFF, 1, buf_avail, b, bb0, limit) - 1;
-					if (len_test < 2) return;
-					const uint32_t st2 = DpEnc::st_lit(st);
-					const uint32_t psn = (pos + 1) & pos_mask;
-					const uint32_t pr_ = c1 + S.pb[st2][psn][1].x + H.len_price(1, len_test, psn);
-					const uint32_t offset = c + 1 + len_test;
-					if (lane == 0) {
-						atomicMax(&S.len_end_sh, offset);
-						uint4 *s = &rg[offset & rmask];
-						const uint4 old = *s;
-						// applied after some of this node's own later classes: it precedes them, so it also wins ties against them
-						if (pr_ < old.x || (late && pr_ == old.x && DP_SRC(offset, old.z) == c))
-							*s = make_uint4(pr_, 0, DP_META(len_test, 1u, 0u, (uint32_t)bb0[1 + len_test]), 0);
-					}
-					__syncwarp();
-				};
-
 				if (!rare) {
-					if (!near_done) wave(0, 3);          // only plain lengths 2 and 3 can land here
-					if (!lr_near && !near_done) {         // (with near_done and no lr_near the flag is out already)
+					if (!near_done) {                     // only plain lengths 2 and 3 can land here
+						wave(0, 3);
 						__syncwarp(); DP_RELEASE();
 						if (lane == 0) S.ph[k] = (want << 2) | 1u;
 					}
-					// the far classes are only worked out here (pushed in the waves below), so they overlap the wait for the
-					// chain warp's verdict on slot c + 1 that "literal + rep0" needs
 					far_classes();
-					lit_rep0(true);
-					if (lr_near) {
-						__syncwarp(); DP_RELEASE();
-						if (lane == 0) S.ph[k] = (want << 2) | 1u;
-					}
 					{ DP_T(w2); if (lane == 0 && w == 0) { DP_ACC(8, w0, w1); DP_ACC(9, w1, w2); DP_CNT(10); } }
 					wave(3, 8);
 					__syncwarp(); DP_RELEASE();
@@ -1244,7 +1266,6 @@ __device__ inline void xzb_dp_worker_main(DS &S, DpEnc &H, const uint32_t w)
 					// uncommon shapes (a second rep matches, very long candidates, > 32 matches): everything in the
 					// reference's order in one go
 					far_classes();
-					lit_rep0(near_done);
 #pragma unroll
 					for (uint32_t ri = 0; ri < XZB_REPS; ++ri) {
 						const uint32_t len_test = rlen[ri];
@@ -1331,6 +1352,43 @@ __device__ inline void xzb_dp_worker_main(DS &S, DpEnc &H, const uint32_t w)
 			__syncwarp(); DP_RELEASE();
 			if (lane == 0) S.ph[k] = (want << 2) | 3u;
 			{ DP_T(w3); if (lane == 0 && w == 0) { DP_ACC(11, w1, w3); DP_ACC(12, wp, w0); } }
+			// "literal + rep0" (:562-597) last: it is pushed only if literal / short rep did not take slot c + 1.  It comes
+			// before this worker starts node c + W (near_old and wait_deadlines rely on that).  In the reference it precedes
+			// the node's other classes, so it wins ties against their entries; against older nodes' entries it loses them.
+			if (lr_len != 0) {
+				uint32_t nv;
+				__syncwarp();
+				for (;;) {
+					nv = __shfl_sync(WFULL, S.nil_node, 0);
+					if ((nv >> 17) == (want >> 16) && ((nv >> 1) & 0xFFFF) >= c) break;
+					if (__shfl_sync(WFULL, (uint32_t)(S.seg_epoch != my_epoch || S.m_exit), 0)) { gone = true; break; }
+				}
+				if (gone) break;
+				// the flag of node c itself; a later value means the chain warp is already past c + 1: read ours from the link
+				bool nil;
+				DP_ACQUIRE();
+				if (((nv >> 1) & 0xFFFF) == c) nil = (nv & 1) != 0;
+				else { const uint32_t m1 = S.o_meta[c + 1]; nil = DP_FLAGS(m1) == 0 && DP_D1(m1) == 1; }
+				if (!nil) {
+					const uint32_t c1 = S.n_c1[k];
+					const uint32_t psn = (pos + 1) & H.pos_mask;
+					const uint32_t pr_ = c1 + S.pb[DpEnc::st_lit(st)][psn][1].x + H.len_price(1, lr_len, psn);
+					const uint32_t offset = c + 1 + lr_len;
+					if (lane == 0) {
+						DP_CNTA(60);
+						// only for a pushed candidate: len_end decides where the segment ends
+						const uint32_t le_was = atomicMax(&S.len_end_sh, offset);
+						if (le_was <= c + 1) DP_CNTA(61);   // without it the segment would end at c + 1
+						(void)le_was;
+						uint4 *s = &rg[offset & rmask];
+						const uint4 old = *s;
+						if (pr_ < old.x || (pr_ == old.x && DP_SRC(offset, old.z) == c))
+							*s = make_uint4(pr_, 0, DP_META(lr_len, 1u, 0u, (uint32_t)(b - hr[0] - 1)[1 + lr_len]), 0);
+					}
+				}
+				__syncwarp(); DP_RELEASE();
+				if (lane == 0) dp_sts64(&S.lr[c & 31], make_uint2(want + 1, 0u));
+			}
 		}
 		// this segment is over for this worker: wait until the chain warp says so, then report idle
 		while (S.seg_stop == DP_NONE && S.seg_epoch == my_epoch && !S.m_exit) __nanosleep(50);

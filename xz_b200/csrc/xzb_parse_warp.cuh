@@ -231,8 +231,7 @@ struct WarpEncT {
 	}
 	__device__ __forceinline__ void put_match(uint32_t i, const xzb_pair v)
 	{
-		S.m_len[i] = (uint16_t)XZB_PAIR_LEN(v.len); S.m_len2[i] = (uint16_t)XZB_PAIR_LEN2(v.len);
-		S.m_mb[i] = (uint8_t)XZB_PAIR_MB(v.len); S.m_dist[i] = v.dist;
+		S.m_len[i] = (uint16_t)XZB_PAIR_LEN(v.len); S.m_dist[i] = v.dist;
 	}
 	__device__ __forceinline__ void mf_skip(uint32_t amount) { read_pos += amount; read_ahead += amount; }
 
@@ -885,8 +884,7 @@ struct FS {
 	alignas(16) xzb_pair ring_mp[32][8];
 	uint32_t ring_mh[32];
 	uint32_t m_dist[XZB_MATCH_LEN_MAX + 1];
-	uint16_t m_len[XZB_MATCH_LEN_MAX + 1], m_len2[XZB_MATCH_LEN_MAX + 1];
-	uint8_t m_mb[XZB_MATCH_LEN_MAX + 1 + 2];
+	uint16_t m_len[XZB_MATCH_LEN_MAX + 1];
 	xzb_prob probs[PI_TOTAL + 2];
 	alignas(8) uint16_t rc_bits[72];
 	volatile uint64_t f_tag[XZB_FRING];
